@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Flagship benchmark: bloom-560m training tokens/s (TP2 x DP, weak scaling) on N B200s.
+"""Flagship benchmark: bloom-560m training tokens/s (TP2 x DP, weak scaling) on N H100s.
 
     python bench.py --gpus 1 --steps 10 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
@@ -7,6 +7,7 @@
     python bench.py --impl reference ...      # the unmodified reference (baseline/_ref) on the same config
     python bench.py --gpus 2 --hf             # our arm fed with a transformers BloomForCausalLM (the reference's input)
     python bench.py --device cpu --model bloom-tiny --seq-len 64 --batch-per-gpu 2 --gpus 2    # dry run of this script
+    python bench.py --gpus 1 --steps 10 --dump-outputs /tmp/out   # + what the last timed step computed, as .npy
 
 Metric/config follow BASELINE.json: bloom-560m, seq 1024, bf16, synthetic token ids, random-init
 weights, Adam; N=1 -> TP1xDP1, N>=2 -> TP2 x DP(N/2); per-GPU work is fixed (weak scaling):
@@ -55,7 +56,7 @@ def _env_defaults():
 
 def _peak_mem_gb(torch, args):
     """Peak bytes this rank's caching allocator handed out (GiB; the NVLink workspaces, mapped with the VMM API, are not
-    the allocator's and not counted).  Informational: how far the config is from the 180 GB of a B200."""
+    the allocator's and not counted).  Informational: how far the config is from the 80 GB of an H100."""
     try:
         if args.device == "cuda" and torch.cuda.is_available():
             return round(torch.cuda.max_memory_allocated() / 2**30, 3)
@@ -144,7 +145,7 @@ def config_of(args, tp, pp, dp):
         "parallelism": f"tp{tp}" + (f"pp{pp}(1f1b,{args.microbatches}mb)" if pp > 1 else "") + f"dp{dp}"
         + ("+zero1" if dp > 1 else "") + (f"+moe{args.experts}e" if args.experts > 0 else ""),
         "optimizer": "Adam", "batch_per_gpu": args.batch_per_gpu,
-        "l2": "no explicit flush: per-step working set (weights + activations, several GB) >> 126 MB L2",
+        "l2": "no explicit flush: per-step working set (weights + activations, several GB) >> 50 MB L2",
     }
 
 
@@ -386,6 +387,7 @@ def run_ours(args):
         loss.backward()
         optim.step()
         last["loss"] = loss.item()  # device -> host read of the step's result (0 on non-final pipeline stages)
+        last["loss_tensor"] = loss.detach()
 
     for i in range(args.warmup):
         step_e2e(i)
@@ -438,9 +440,43 @@ def run_ours(args):
         result["mfu_vs_measured_sustained"] = flops / (ms_dev / args.steps / 1e3) / (peaks["bf16_tflops_sustained"] * 1e12)
     except Exception:
         pass
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, torch, dist, model, last["loss_tensor"], rank)
     if rank == 0:
         print(json.dumps(result), flush=True)
     ctx.destroy()
+
+
+DUMP_PARAM_SAMPLE = 4 * 2**20  # parameter elements kept per dump (16 MB as float32)
+
+
+def dump_outputs(out_dir, torch, dist, model, loss, rank):
+    """What the last timed step handed back to its caller, as ``<out_dir>/<name>.npy``: the step's loss (float64, summed
+    over ranks like the numerics self-check) and the parameters it left behind (float32).  Parameters are a fixed,
+    seeded sample (DUMP_PARAM_SAMPLE elements shared out over the ranks) of each rank's parameters in
+    ``named_parameters`` order, so two builds of the project run with the same arguments compare array for array."""
+    import numpy as np
+
+    world = dist.get_world_size() if dist.is_initialized() else 1
+    params = [p.detach() for _, p in model.named_parameters()]
+    sizes = torch.tensor([p.numel() for p in params])
+    starts = torch.cumsum(sizes, 0) - sizes
+    gen = torch.Generator().manual_seed(2024)
+    idx = torch.randint(0, int(sizes.sum()), (DUMP_PARAM_SAMPLE // world,), generator=gen).sort().values
+    which = torch.searchsorted(starts, idx, right=True) - 1   # the parameter each sampled element lives in
+    parts = []
+    for i in torch.unique_consecutive(which).tolist():   # gathered per parameter: no concatenated copy of the model
+        local = (idx[which == i] - starts[i]).to(params[i].device)
+        parts.append(params[i].reshape(-1)[local].float().cpu())
+    sample = torch.cat(parts).numpy()
+    loss = loss.double().reshape(1)
+    if world > 1:
+        dist.all_reduce(loss)
+    os.makedirs(out_dir, exist_ok=True)
+    suffix = "" if rank == 0 else f"_rank{rank}"
+    np.save(os.path.join(out_dir, f"params_sample{suffix}.npy"), sample)
+    if rank == 0:
+        np.save(os.path.join(out_dir, "loss.npy"), loss.cpu().numpy())
 
 
 # --------------------------------------------------------------------------------------------
@@ -569,6 +605,7 @@ def run_reference(args):
         loss.backward()
         optim.step()
         last["loss"] = loss.item()
+        last["loss_tensor"] = loss.detach()
 
     for i in range(args.warmup):
         step_e2e(i)
@@ -599,6 +636,8 @@ def run_reference(args):
     result["peak_mem_gb"] = _peak_mem_gb(torch, args)
     if note is not None:
         result["note"] = note
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, torch, dist, model, last["loss_tensor"], rank)
     if rank == 0:
         print(json.dumps(result), flush=True)
     try:
@@ -631,6 +670,9 @@ def main():
                     help="where the random weights are created (auto: on the GPU for the >= 1.7B configs)")
     ap.add_argument("--device", default="cuda", choices=["cuda", "cpu"],
                     help="cpu: dry run of this script on gloo with a tiny model (no benchmark value)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's loss and a seeded sample of the parameters it "
+                         "produced to DIR/<name>.npy (both arms)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     _env_defaults()

@@ -4,7 +4,7 @@ TensorParallel x DataParallel + ZeRO-1, and every step's loss is printed next to
 single-process model trained on the same global batch.
 
     torchrun --standalone --nnodes=1 --nproc-per-node 4 examples/convergence_hybrid.py --tp 2 --dp 2 --steps 60
-    (CPU: add --backend gloo; GPUs: --backend nccl uses the sm_100a kernels in bf16)
+    (CPU: add --backend gloo; GPUs: --backend nccl uses the sm_90a kernels in bf16)
 """
 import argparse
 import os

@@ -4,7 +4,7 @@ own synthetic shard with its own FusedAdam; every --inner-steps steps the worker
 Nesterov SGD moves the shared parameters.
 
     torchrun --standalone --nnodes=1 --nproc-per-node 4 examples/diloco.py --tp 2 --workers 2 --backend gloo   # CPU
-    torchrun --standalone --nnodes=1 --nproc-per-node 8 examples/diloco.py --tp 2 --workers 4                  # B200s
+    torchrun --standalone --nnodes=1 --nproc-per-node 8 examples/diloco.py --tp 2 --workers 4                  # H100s
 """
 import argparse
 import os

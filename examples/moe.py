@@ -30,7 +30,7 @@ if __name__ == "__main__":
     model = BloomForCausalLM(cfg)
     router = Top1Router(SwitchNoisePolicy(), args.experts, cfg.hidden_size, expert_capacity=(1.25, 2.0))
     gpu = args.backend == "nccl"
-    if gpu:  # bf16 on the B200 path: router kernel + NVLink dispatch + grouped tcgen05 expert GEMMs
+    if gpu:  # bf16 on the GPU path: router kernel + NVLink dispatch + grouped wgmma expert GEMMs
         model, router = model.to(torch.bfloat16), router.to(torch.bfloat16)
     model = ExpertParallel(model, args.experts, mapping=[0, 2], router=router, parallel_context=ctx).parallelize()
     model = TensorParallel(model, ctx).parallelize()

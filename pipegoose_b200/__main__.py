@@ -1,6 +1,6 @@
 """``python -m pipegoose_b200`` — what this installation can do on this machine (paste it into a bug report).
 
-Prints the package / torch / CUDA versions, whether the sm_100a extension is built and loads, the GPUs and whether they can
+Prints the package / torch / CUDA versions, whether the sm_90a extension is built and loads, the GPUs and whether they can
 address each other's memory (the NVLink engines need peer access), the ``PIPEGOOSE_B200_*`` switches that are set, and the
 launcher environment.  Never raises: every probe that fails is reported as such.
 """
@@ -35,7 +35,7 @@ def main() -> int:
                                      " (CPU only: gloo paths and PyTorch fallbacks of every op)"))
     if n:
         _probe("compute capability", lambda: ", ".join(sorted({"sm_%d%d" % torch.cuda.get_device_capability(i) for i in range(n)}))
-               + "  (the kernels are sm_100a only)")
+               + "  (the kernels are sm_90a only)")
         _probe("extension loads", lambda: sorted(k for k in dir(__import__("pipegoose_b200.ops", fromlist=["native"]).native())
                                                   if not k.startswith("_"))[:4] + ["..."])
         if n > 1:

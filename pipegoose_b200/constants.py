@@ -16,8 +16,14 @@ PIPELINE_MIN_WORKERS = 1
 PIPELINE_MAX_WORKERS = 1
 JOB_KEY_LENGTH = 15
 
-# B200 facts used by heuristics (grid sizing, bucket sizing)
-B200_NUM_SMS = 148
-B200_L2_BYTES = 126 * 1024 * 1024
-B200_HBM_BYTES = 180 * 1024**3
+# H100 SXM facts used by heuristics (grid sizing, bucket sizing, layout planning) and as roofline denominators
+H100_NUM_SMS = 132
+H100_L2_BYTES = 50 * 1024 * 1024
+H100_HBM_BYTES = 80 * 1024**3
+H100_BF16_DENSE_FLOPS = 989e12     # data sheet, dense bf16 at the 700 W limit (not reached)
+H100_NVLINK_BYTES_PER_S = 450e9    # NVLink4: 900 GB/s bidirectional per GPU = 450 GB/s per direction (data sheet)
+# the names these constants had before the port (same values), for code that imports them
+B200_NUM_SMS = H100_NUM_SMS
+B200_L2_BYTES = H100_L2_BYTES
+B200_HBM_BYTES = H100_HBM_BYTES
 MAX_NVLINK_PEERS = 8

@@ -2,7 +2,7 @@
 
 ``FlatModelState`` re-points every parameter of a module at a view of ONE contiguous buffer of
 the model dtype and gives every parameter an fp32 ``main_grad`` view of ONE contiguous gradient
-buffer.  That layout is what the B200 path is built around:
+buffer.  That layout is what the GPU path is built around:
 
 * the wgrad GEMM epilogue accumulates straight into ``param.main_grad`` (no ``.grad`` tensors,
   no bf16->fp32 cast pass);

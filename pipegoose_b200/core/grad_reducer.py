@@ -9,7 +9,7 @@ has its gradient, on a side stream, while backward keeps running.  Modes:
 * ``reduce_scatter``  rank ``r`` ends with slice ``r`` of every bucket (what the fused ZeRO-1
                       optimizer consumes) — half the bytes of an all-reduce
 
-On NVLink-connected B200s the collective is the hand-written peer-memory kernel from
+On NVLink-connected GPUs the collective is the hand-written peer-memory kernel from
 ``pipegoose_b200.ops.comm`` (fused with the 1/dp scale); NCCL/gloo is the fallback.
 """
 from __future__ import annotations

@@ -1,0 +1,662 @@
+// Causal ALiBi flash attention for sm_90a on Bloom's fused QKV layout.
+//
+//   qkv : [B*S, H*3*D] bf16, each row laid out [head][q|k|v][D]      out : [B*S, H*D] bf16
+//   scores = q.k / sqrt(D) + slope[head] * (key_pos - query_pos)  (== slope * key_pos under softmax)
+//
+// Forward: one CTA per (128-query block, head, batch).  A TMA warp streams Q once and K/V blocks
+// through a 2-stage ring; two consumer warpgroups own 64 query rows each and compute S = Q K^T with
+// wgmma (fp32 accumulators in registers), the online softmax in registers (a row is spread over the
+// four threads of a quad), and O += P V with P taken straight from registers as the A operand (the
+// accumulator fragment of S is the A fragment of P).  [S, S] never exists.
+//
+// Backward: one CTA per (128-key block, head, batch) looping over the 64-row query blocks at or below
+// the diagonal.  Two consumer warpgroups own 64 keys each: S^T = K Q^T and dP^T = V dO^T on the tensor
+// cores, P^T / dS^T recomputed in registers, dV += P^T dO and dK += dS^T Q with P^T / dS^T as register
+// A operands (dV, dK accumulate in registers across the loop), and the warpgroup's share of
+// dQ = dS K (its 64 keys) from dS^T staged in shared memory, reduced into an fp32 buffer with
+// red.global.add.
+#include "launch.h"
+#include "pdl_launch.cuh"
+#include "ptx.cuh"
+#include "wgmma.cuh"
+#include <cstdio>
+#include <cstring>
+#include <mutex>
+#include <unordered_map>
+
+namespace pg {
+
+int make_tmap_bf16_2d(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld,
+                      uint32_t box_rows, uint32_t box_cols);
+
+constexpr int ATT_BM = 128;      // queries per forward CTA
+constexpr int ATT_BN = 128;      // keys per block
+constexpr int ATT_BWD_BM = 64;   // queries per backward step
+constexpr int kAttThreads = 384;  // warpgroup 0: warp 0 TMA; warpgroups 1, 2: consumers
+constexpr float kLog2e = 1.4426950408889634f;
+
+PG_DEVICE float fast_exp2(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+
+PG_DEVICE void red_add_v2_f32(float* addr, float a, float b) {
+  asm volatile("red.relaxed.gpu.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
+}
+
+// A operand (k16 slice kk) of a bf16 product from an fp32 accumulator fragment (columns 16 kk .. 16 kk + 15)
+template <int R>
+PG_DEVICE void acc_to_a(const float (&d)[R], int kk, uint32_t (&a)[4]) {
+  a[0] = pack_bf16x2(d[8 * kk + 0], d[8 * kk + 1]);
+  a[1] = pack_bf16x2(d[8 * kk + 2], d[8 * kk + 3]);
+  a[2] = pack_bf16x2(d[8 * kk + 4], d[8 * kk + 5]);
+  a[3] = pack_bf16x2(d[8 * kk + 6], d[8 * kk + 7]);
+}
+
+constexpr int kAttRegsLight = 24;
+constexpr int kAttRegsConsumer = 240;
+
+template <int D>
+struct AttFwdCfg {
+  static constexpr int kTileBytes = ATT_BM * D * 2;  // Q, K or V tile: D/64 atoms of [128 rows x 128 B]
+  static constexpr int kStages = 2;
+  static constexpr int kSmemBytes = kTileBytes * (1 + 2 * kStages) + 256 + 1024 /*align*/;
+};
+
+struct AttFwdArgs {
+  __nv_bfloat16* out;
+  float* lse;  // [B, H, S] natural log
+  const float* slopes;
+  int B, S, H, ld_out;
+  float scale_log2;  // log2(e) / sqrt(D)
+};
+
+template <int D>
+__global__ void __launch_bounds__(kAttThreads, 1)
+    attention_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const AttFwdArgs args) {
+  using Cfg = AttFwdCfg<D>;
+  constexpr int ST = Cfg::kStages;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint8_t* sQ = smem;
+  uint8_t* sK = sQ + Cfg::kTileBytes;
+  uint8_t* sV = sK + ST * Cfg::kTileBytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + ST * Cfg::kTileBytes);
+  uint64_t* q_full = bars;            // 1
+  uint64_t* kv_full = bars + 1;       // ST
+  uint64_t* kv_empty = kv_full + ST;  // ST
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) pdl_launch_dependents();
+  const int num_qb = (args.S + ATT_BM - 1) / ATT_BM;
+  const int qb = num_qb - 1 - blockIdx.x;  // longest (most key blocks) first
+  const int head = blockIdx.y, batch = blockIdx.z;
+  const int num_kb = qb + 1;
+  const int row0 = batch * args.S + qb * ATT_BM;  // global row of the first query
+  const int col_q = head * 3 * D, col_k = col_q + D, col_v = col_q + 2 * D;
+
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tm_qkv);
+    mbar_init(q_full, 1);
+    for (int i = 0; i < ST; ++i) {
+      mbar_init(&kv_full[i], 1);
+      mbar_init(&kv_empty[i], 2);  // one arrival per consumer warpgroup
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();  // prologue above overlapped the predecessor; Q/K/V are read below
+
+  if (warp < 4) {
+    setmaxnreg_dec<kAttRegsLight>();
+    if (warp == 0) {
+      // ===================== TMA producer =====================
+      if (lane == 0) {
+        mbar_arrive_expect_tx(q_full, Cfg::kTileBytes);
+#pragma unroll
+        for (int a = 0; a < D / 64; ++a) tma_load_2d(sQ + a * 16384, &tm_qkv, q_full, col_q + a * 64, row0);
+      }
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int j = 0; j < num_kb; ++j) {
+        mbar_wait(&kv_empty[stage], phase ^ 1);
+        if (lane == 0) {
+          const int krow = batch * args.S + j * ATT_BN;
+          mbar_arrive_expect_tx(&kv_full[stage], 2 * Cfg::kTileBytes);
+#pragma unroll
+          for (int a = 0; a < D / 64; ++a) {
+            tma_load_2d(sK + stage * Cfg::kTileBytes + a * 16384, &tm_qkv, &kv_full[stage], col_k + a * 64, krow);
+            tma_load_2d(sV + stage * Cfg::kTileBytes + a * 16384, &tm_qkv, &kv_full[stage], col_v + a * 64, krow);
+          }
+        }
+        __syncwarp();
+        if (++stage == ST) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<kAttRegsConsumer>();
+  // ===================== consumers: warpgroup wg owns query rows [64 wg, 64 wg + 64) =====================
+  const int wg = (warp >> 2) - 1, wl = warp & 3;
+  const int tid_wg = threadIdx.x & 127;
+  const int t4 = lane & 3;
+  int qpos[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) qpos[hh] = qb * ATT_BM + 64 * wg + 16 * wl + (lane >> 2) + 8 * hh;
+  const float slope2 = args.slopes[head] * kLog2e;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  float s[ATT_BN / 2];
+  float o[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+  const uint32_t aQ = smem_u32(sQ) + wg * 8192;
+  mbar_wait(q_full, 0);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int j = 0; j < num_kb; ++j) {
+    mbar_wait(&kv_full[stage], phase);
+    const uint32_t aK = smem_u32(sK + stage * Cfg::kTileBytes), aV = smem_u32(sV + stage * Cfg::kTileBytes);
+    // S = Q K^T
+    wgmma_fence_regs(s);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < D / 16; ++k) {
+      const uint32_t off = (k >> 2) * 16384 + (k & 3) * 32;
+      Wgmma<ATT_BN, 0, 0>::mma(s, make_wgmma_desc_sw128(aQ + off, 0, 1024), make_wgmma_desc_sw128(aK + off, 0, 1024),
+                               k != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    // x = s*scale_log2 + slope2*(kpos - qpos); the causal mask only matters on the diagonal block
+    const bool diag = (j == qb);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const float bias0 = slope2 * static_cast<float>(j * ATT_BN - qpos[hh]);
+      const int lim = qpos[hh] - j * ATT_BN;  // column c is visible iff c <= lim
+      float mx = -INFINITY;
+#pragma unroll
+      for (int jn = 0; jn < ATT_BN / 8; ++jn) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = 8 * jn + 2 * t4 + e;
+          float x = fmaf(s[4 * jn + 2 * hh + e], args.scale_log2, fmaf(slope2, static_cast<float>(col), bias0));
+          if (diag && col > lim) x = -INFINITY;
+          s[4 * jn + 2 * hh + e] = x;
+          mx = fmaxf(mx, x);
+        }
+      }
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[hh], mx);
+      const float alpha = fast_exp2(m_run[hh] - m_new);  // m_run = -inf on the first block -> 0
+      float rs = 0.f;
+#pragma unroll
+      for (int jn = 0; jn < ATT_BN / 8; ++jn) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float p = fast_exp2(s[4 * jn + 2 * hh + e] - m_new);
+          s[4 * jn + 2 * hh + e] = p;
+          rs += p;
+        }
+      }
+      l_run[hh] = l_run[hh] * alpha + rs;  // per-thread partial over its columns; the quad is summed at the end
+      m_run[hh] = m_new;
+#pragma unroll
+      for (int jn = 0; jn < D / 8; ++jn) {
+        o[4 * jn + 2 * hh] *= alpha;
+        o[4 * jn + 2 * hh + 1] *= alpha;
+      }
+    }
+    // O += P V   (P from registers, packed before the fence so that no wgmma waits on a register write; V MN-major:
+    // D/64 atoms of [128 keys x 64] 16 KB apart)
+    uint32_t pa[ATT_BN / 16][4];
+#pragma unroll
+    for (int kk = 0; kk < ATT_BN / 16; ++kk) acc_to_a(s, kk, pa[kk]);
+    wgmma_fence_regs(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < ATT_BN / 16; ++kk)
+      WgmmaRS<D, 1>::mma(o, pa[kk], make_wgmma_desc_sw128(aV + kk * 2048, 16384, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    if (tid_wg == 0) mbar_arrive(&kv_empty[stage]);
+    if (++stage == ST) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    float l = l_run[hh];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv_l = 1.f / l;
+    if (qpos[hh] < args.S) {
+      __nv_bfloat16* orow = args.out + static_cast<size_t>(batch * args.S + qpos[hh]) * args.ld_out + head * D;
+#pragma unroll
+      for (int jn = 0; jn < D / 8; ++jn)
+        *reinterpret_cast<uint32_t*>(orow + 8 * jn + 2 * t4) =
+            pack_bf16x2(o[4 * jn + 2 * hh] * inv_l, o[4 * jn + 2 * hh + 1] * inv_l);
+      if (t4 == 0)
+        args.lse[(static_cast<size_t>(batch) * args.H + head) * args.S + qpos[hh]] =
+            (m_run[hh] + log2f(l)) * 0.6931471805599453f;
+    }
+  }
+}
+
+// -----------------------------------------------------------------------------------------------
+// backward
+// -----------------------------------------------------------------------------------------------
+// delta[b,h,i] = sum_d dO[i,d] * O[i,d].  One warp per token row: every lane loads 16-byte chunks of the
+// [H*D] row (fully coalesced), the D/8 lanes that share a head reduce with shuffles.
+__global__ void __launch_bounds__(256) attention_delta_kernel(const __nv_bfloat16* __restrict__ dout,
+                                                              const __nv_bfloat16* __restrict__ out,
+                                                              float* __restrict__ delta, int B, int S, int H,
+                                                              int D) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (row >= B * S) return;
+  const int cph = D / 8;                 // 16-byte chunks (= lanes) per head: 8 or 16
+  const int nchunks = H * cph;
+  const __nv_bfloat16* a = dout + static_cast<size_t>(row) * H * D;
+  const __nv_bfloat16* b = out + static_cast<size_t>(row) * H * D;
+  const int bidx = row / S, spos = row % S;
+  for (int c0 = 0; c0 < nchunks; c0 += 32) {
+    const int c = c0 + lane;
+    float s = 0.f;
+    if (c < nchunks) {
+      const uint4 x = ld_global_nc_v4(a + c * 8), y = ld_global_nc_v4(b + c * 8);
+      const uint32_t xw[4] = {x.x, x.y, x.z, x.w}, yw[4] = {y.x, y.y, y.z, y.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 f = unpack_bf16x2(xw[j]), g = unpack_bf16x2(yw[j]);
+        s += f.x * g.x + f.y * g.y;
+      }
+    }
+    for (int o = cph >> 1; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (c < nchunks && (lane & (cph - 1)) == 0) {
+      const int head = c / cph;
+      delta[(static_cast<size_t>(bidx) * H + head) * S + spos] = s;
+    }
+  }
+}
+
+template <int D>
+struct AttBwdCfg {
+  static constexpr int kKVBytes = ATT_BN * D * 2;     // K or V tile: D/64 atoms of [128 keys x 128 B]
+  static constexpr int kQBytes = ATT_BWD_BM * D * 2;  // Q or dO tile: D/64 atoms of [64 queries x 128 B]
+  static constexpr int kQStages = 2;
+  static constexpr int kdSBytes = ATT_BN * ATT_BWD_BM * 2;  // dS^T [128 keys x 64 queries], one swizzled atom
+  static constexpr int kSmemBytes = 2 * kKVBytes + 2 * kQStages * kQBytes + kdSBytes + 256 + 1024 /*align*/;
+};
+
+struct AttBwdArgs {
+  const float* lse;
+  const float* delta;
+  const float* slopes;
+  float* dq_acc;            // [B*S, H*D] fp32, zero-initialised
+  __nv_bfloat16* dqkv;      // [B*S, H*3*D]
+  int B, S, H;
+  float scale, scale_log2;
+};
+
+template <int D>
+__global__ void __launch_bounds__(kAttThreads, 1)
+    attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant__ CUtensorMap tm_q,
+                         const __grid_constant__ CUtensorMap tm_do, const AttBwdArgs args) {
+  using Cfg = AttBwdCfg<D>;
+  constexpr int QS = Cfg::kQStages;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint8_t* sK = smem;
+  uint8_t* sV = sK + Cfg::kKVBytes;
+  uint8_t* sQ = sV + Cfg::kKVBytes;
+  uint8_t* sdO = sQ + QS * Cfg::kQBytes;
+  uint8_t* sdS = sdO + QS * Cfg::kQBytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sdS + Cfg::kdSBytes);
+  uint64_t* kv_full = bars;         // 1
+  uint64_t* q_full = bars + 1;      // QS
+  uint64_t* q_empty = q_full + QS;  // QS
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) pdl_launch_dependents();
+  const int num_qb = (args.S + ATT_BWD_BM - 1) / ATT_BWD_BM;
+  const int jb = blockIdx.x;  // key block
+  const int head = blockIdx.y, batch = blockIdx.z;
+  const int qb0 = jb * (ATT_BN / ATT_BWD_BM);  // first query block that sees these keys
+  const int n_iter = num_qb - qb0;
+  const int col_q = head * 3 * D, col_k = col_q + D, col_v = col_q + 2 * D;
+  const int krow0 = batch * args.S + jb * ATT_BN;
+
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tm_kv);
+    tma_prefetch_desc(&tm_q);
+    tma_prefetch_desc(&tm_do);
+    mbar_init(kv_full, 1);
+    for (int i = 0; i < QS; ++i) {
+      mbar_init(&q_full[i], 1);
+      mbar_init(&q_empty[i], 2);  // one arrival per consumer warpgroup
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();  // prologue above overlapped the predecessor; Q/K/V, dO, lse, delta are read below
+
+  if (warp < 4) {
+    setmaxnreg_dec<kAttRegsLight>();
+    if (warp == 0) {
+      // ===================== TMA producer =====================
+      if (lane == 0) {
+        mbar_arrive_expect_tx(kv_full, 2 * Cfg::kKVBytes);
+#pragma unroll
+        for (int a = 0; a < D / 64; ++a) {
+          tma_load_2d(sK + a * 16384, &tm_kv, kv_full, col_k + a * 64, krow0);
+          tma_load_2d(sV + a * 16384, &tm_kv, kv_full, col_v + a * 64, krow0);
+        }
+      }
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int it = 0; it < n_iter; ++it) {
+        const int qrow = batch * args.S + (qb0 + it) * ATT_BWD_BM;
+        mbar_wait(&q_empty[stage], phase ^ 1);
+        if (lane == 0) {
+          mbar_arrive_expect_tx(&q_full[stage], 2 * Cfg::kQBytes);
+#pragma unroll
+          for (int a = 0; a < D / 64; ++a) {
+            tma_load_2d(sQ + stage * Cfg::kQBytes + a * 8192, &tm_q, &q_full[stage], col_q + a * 64, qrow);
+            tma_load_2d(sdO + stage * Cfg::kQBytes + a * 8192, &tm_do, &q_full[stage], head * D + a * 64, qrow);
+          }
+        }
+        __syncwarp();
+        if (++stage == QS) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<kAttRegsConsumer>();
+  // ===================== consumers: warpgroup wg owns keys [64 wg, 64 wg + 64) of the block =====================
+  const int wg = (warp >> 2) - 1, wl = warp & 3;
+  const int tid_wg = threadIdx.x & 127;
+  const int t4 = lane & 3;
+  int kr[2], kpos[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    kr[hh] = 64 * wg + 16 * wl + (lane >> 2) + 8 * hh;  // key row inside the block
+    kpos[hh] = jb * ATT_BN + kr[hh];
+  }
+  const float slope2 = args.slopes[head] * kLog2e;
+  const uint32_t aK = smem_u32(sK) + wg * 8192, aV = smem_u32(sV) + wg * 8192;
+  const uint32_t adS = smem_u32(sdS);
+  float dv[D / 2], dk[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) {
+    dv[i] = 0.f;
+    dk[i] = 0.f;
+  }
+  mbar_wait(kv_full, 0);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int it = 0; it < n_iter; ++it) {
+    const int qb = qb0 + it;
+    mbar_wait(&q_full[stage], phase);
+    const uint32_t aQ = smem_u32(sQ + stage * Cfg::kQBytes), adO = smem_u32(sdO + stage * Cfg::kQBytes);
+    float st[ATT_BWD_BM / 2], dpt[ATT_BWD_BM / 2];
+    // S^T = K Q^T, dP^T = V dO^T   (64 keys x 64 queries, contraction over D)
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < D / 16; ++k) {
+      const uint32_t okv = (k >> 2) * 16384 + (k & 3) * 32, oq = (k >> 2) * 8192 + (k & 3) * 32;
+      Wgmma<ATT_BWD_BM, 0, 0>::mma(st, make_wgmma_desc_sw128(aK + okv, 0, 1024), make_wgmma_desc_sw128(aQ + oq, 0, 1024),
+                                   k != 0 ? 1u : 0u);
+    }
+#pragma unroll
+    for (int k = 0; k < D / 16; ++k) {
+      const uint32_t okv = (k >> 2) * 16384 + (k & 3) * 32, oq = (k >> 2) * 8192 + (k & 3) * 32;
+      Wgmma<ATT_BWD_BM, 0, 0>::mma(dpt, make_wgmma_desc_sw128(aV + okv, 0, 1024), make_wgmma_desc_sw128(adO + oq, 0, 1024),
+                                   k != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(st);
+    wgmma_fence_regs(dpt);
+    // p = exp2(s*scale_log2 + slope2*(kpos-qpos) - lse2); dS = p * (dP - delta) * scale.  Masked (key after query)
+    // and out-of-sequence queries get p = 0.
+#pragma unroll
+    for (int jn = 0; jn < ATT_BWD_BM / 8; ++jn) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int qpos = qb * ATT_BWD_BM + 8 * jn + 2 * t4 + e;
+        const bool q_ok = qpos < args.S;
+        const size_t stat_idx = (static_cast<size_t>(batch) * args.H + head) * args.S + qpos;
+        const float lse2 = q_ok ? args.lse[stat_idx] * kLog2e : 0.f;
+        const float nds = q_ok ? -args.delta[stat_idx] * args.scale : 0.f;
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int i = 4 * jn + 2 * hh + e;
+          float p = fast_exp2(fmaf(st[i], args.scale_log2, fmaf(slope2, static_cast<float>(kpos[hh] - qpos), -lse2)));
+          if (!q_ok || kpos[hh] > qpos) p = 0.f;
+          st[i] = p;
+          dpt[i] = p * fmaf(dpt[i], args.scale, nds);
+        }
+      }
+    }
+    // dS^T (bf16) -> shared memory, [128 keys x 64 queries] with the 128-byte swizzle, for the dQ product below
+#pragma unroll
+    for (int jn = 0; jn < ATT_BWD_BM / 8; ++jn) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = kr[hh];
+        const uint32_t off = r * 128 + ((jn ^ (r & 7)) << 4) + t4 * 4;
+        *reinterpret_cast<uint32_t*>(sdS + off) = pack_bf16x2(dpt[4 * jn + 2 * hh], dpt[4 * jn + 2 * hh + 1]);
+      }
+    }
+    // dV += P^T dO ; dK += dS^T Q   (contraction over the 64 queries; dO / Q MN-major: D/64 atoms 8 KB apart)
+    uint32_t pa[ATT_BWD_BM / 16][4], dsa[ATT_BWD_BM / 16][4];  // packed before the fence (see the forward)
+#pragma unroll
+    for (int kk = 0; kk < ATT_BWD_BM / 16; ++kk) {
+      acc_to_a(st, kk, pa[kk]);
+      acc_to_a(dpt, kk, dsa[kk]);
+    }
+    wgmma_fence_regs(dv);
+    wgmma_fence_regs(dk);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < ATT_BWD_BM / 16; ++kk)
+      WgmmaRS<D, 1>::mma(dv, pa[kk], make_wgmma_desc_sw128(adO + kk * 2048, 8192, 1024), 1u);
+#pragma unroll
+    for (int kk = 0; kk < ATT_BWD_BM / 16; ++kk)
+      WgmmaRS<D, 1>::mma(dk, dsa[kk], make_wgmma_desc_sw128(aQ + kk * 2048, 8192, 1024), 1u);
+    wgmma_commit();
+    fence_proxy_async_smem();  // dS^T writes -> async-proxy (wgmma) reads
+    named_bar_sync(2 + wg, 128);
+    // this warpgroup's share of dQ = dS K: its 64 keys, 64 output columns per pass.  A = dS (MN-major: queries
+    // contiguous in the dS^T rows), B = K (MN-major: D contiguous)
+#pragma unroll
+    for (int pass = 0; pass < D / 64; ++pass) {
+      float dq[32];
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+        Wgmma<64, 1, 1>::mma(dq, make_wgmma_desc_sw128(adS + wg * 8192 + kk * 2048, 8192, 1024),
+                             make_wgmma_desc_sw128(aK + pass * 16384 + kk * 2048, 16384, 1024), kk != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(dq);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int qpos = qb * ATT_BWD_BM + 16 * wl + (lane >> 2) + 8 * hh;
+        if (qpos < args.S) {
+          float* dq_row = args.dq_acc + static_cast<size_t>(batch * args.S + qpos) * (args.H * D) + head * D + pass * 64;
+#pragma unroll
+          for (int jn = 0; jn < 8; ++jn) red_add_v2_f32(dq_row + 8 * jn + 2 * t4, dq[4 * jn + 2 * hh], dq[4 * jn + 2 * hh + 1]);
+        }
+      }
+    }
+    wgmma_fence_regs(dv);
+    wgmma_fence_regs(dk);
+    // every wgmma of this step has retired (the waits above cover the dV / dK group): Q / dO / dS^T are free
+    named_bar_sync(2 + wg, 128);
+    if (tid_wg == 0) mbar_arrive(&q_empty[stage]);
+    if (++stage == QS) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+  // dK, dV of this key block
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    if (kpos[hh] >= args.S) continue;
+    __nv_bfloat16* dk_row = args.dqkv + static_cast<size_t>(batch * args.S + kpos[hh]) * (args.H * 3 * D) + col_k;
+    __nv_bfloat16* dv_row = dk_row + D;
+#pragma unroll
+    for (int jn = 0; jn < D / 8; ++jn) {
+      *reinterpret_cast<uint32_t*>(dk_row + 8 * jn + 2 * t4) = pack_bf16x2(dk[4 * jn + 2 * hh], dk[4 * jn + 2 * hh + 1]);
+      *reinterpret_cast<uint32_t*>(dv_row + 8 * jn + 2 * t4) = pack_bf16x2(dv[4 * jn + 2 * hh], dv[4 * jn + 2 * hh + 1]);
+    }
+  }
+}
+
+// dq fp32 [rows, H*D] -> bf16 into dqkv[rows, H*3*D] (q slot of every head)
+__global__ void __launch_bounds__(256) attention_dq_convert_kernel(const float* __restrict__ dq,
+                                                                   __nv_bfloat16* __restrict__ dqkv, int64_t rows,
+                                                                   int H, int D) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int64_t idx = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) * 8;
+  const int64_t total = rows * H * D;
+  if (idx >= total) return;
+  const int64_t row = idx / (H * D);
+  const int rem = static_cast<int>(idx % (H * D));
+  const int head = rem / D, d = rem % D;
+  const float4 a = *reinterpret_cast<const float4*>(dq + idx);
+  const float4 b = *reinterpret_cast<const float4*>(dq + idx + 4);
+  st_global_v4(dqkv + row * (H * 3 * D) + head * 3 * D + d,
+               make_uint4(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w), pack_bf16x2(b.x, b.y), pack_bf16x2(b.z, b.w)));
+}
+
+}  // namespace pg
+
+using namespace pg;
+
+static int att_tmap(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+  struct Key {
+    const void* p;
+    uint64_t r, c;
+    uint32_t b;
+    bool operator==(const Key& o) const { return p == o.p && r == o.r && c == o.c && b == o.b; }
+  };
+  struct H {
+    size_t operator()(const Key& k) const {
+      return reinterpret_cast<size_t>(k.p) ^ (k.r * 1315423911u) ^ (k.c << 20) ^ (static_cast<size_t>(k.b) << 40);
+    }
+  };
+  static std::unordered_map<Key, CUtensorMap, H> cache;
+  static std::mutex mu;
+  std::lock_guard<std::mutex> g(mu);
+  Key key{ptr, rows, cols, box_rows};
+  auto it = cache.find(key);
+  if (it != cache.end()) {
+    *out = it->second;
+    return 0;
+  }
+  if (make_tmap_bf16_2d(out, ptr, rows, cols, cols, box_rows, 64) != 0) return -1;
+  if (cache.size() > 4096) cache.clear();
+  cache.emplace(key, *out);
+  return 0;
+}
+
+#define PG_CHECK_LAUNCH(name)                                                       \
+  do {                                                                              \
+    cudaError_t e__ = cudaGetLastError();                                           \
+    if (e__ != cudaSuccess) {                                                       \
+      fprintf(stderr, "pipegoose_b200: %s launch failed: %s\n", name, cudaGetErrorString(e__)); \
+      return -1;                                                                    \
+    }                                                                               \
+  } while (0)
+
+template <int D>
+static int launch_att_fwd(const CUtensorMap& tm, const AttFwdArgs& a, cudaStream_t s) {
+  using Cfg = AttFwdCfg<D>;
+  static bool set = false;
+  if (!set) {
+    if (cudaFuncSetAttribute(attention_fwd_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) != cudaSuccess) return -1;
+    set = true;
+  }
+  dim3 grid((a.S + ATT_BM - 1) / ATT_BM, a.H, a.B);
+  if (launch_pdl(attention_fwd_kernel<D>, grid, dim3(kAttThreads), Cfg::kSmemBytes, s, tm, a) != cudaSuccess) return -1;
+  PG_CHECK_LAUNCH("attention_fwd");
+  return 0;
+}
+
+// softmax_scale <= 0: 1/sqrt(D).  An explicit scale lets a head that was zero-padded to a supported width (e.g. D=80
+// -> 128: the padded columns contribute nothing to Q.K) keep the scale of its true width.
+extern "C" int pg_attention_fwd(const void* qkv, const float* slopes, void* out, float* lse, int B, int S, int H,
+                                int D, float softmax_scale, cudaStream_t s) {
+  if (D != 64 && D != 128) return -1;
+  CUtensorMap tm;
+  if (att_tmap(&tm, qkv, static_cast<uint64_t>(B) * S, static_cast<uint64_t>(H) * 3 * D, ATT_BM) != 0) return -1;
+  AttFwdArgs a;
+  a.out = (__nv_bfloat16*)out;
+  a.lse = lse;
+  a.slopes = slopes;
+  a.B = B; a.S = S; a.H = H;
+  a.ld_out = H * D;
+  a.scale_log2 = kLog2e * (softmax_scale > 0.f ? softmax_scale : 1.0f / sqrtf(static_cast<float>(D)));
+  return D == 64 ? launch_att_fwd<64>(tm, a, s) : launch_att_fwd<128>(tm, a, s);
+}
+
+template <int D>
+static int launch_att_bwd(const CUtensorMap& tkv, const CUtensorMap& tq, const CUtensorMap& tdo, const AttBwdArgs& a,
+                          cudaStream_t s) {
+  using Cfg = AttBwdCfg<D>;
+  static bool set = false;
+  if (!set) {
+    if (cudaFuncSetAttribute(attention_bwd_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) != cudaSuccess) return -1;
+    set = true;
+  }
+  dim3 grid((a.S + ATT_BN - 1) / ATT_BN, a.H, a.B);
+  if (launch_pdl(attention_bwd_kernel<D>, grid, dim3(kAttThreads), Cfg::kSmemBytes, s, tkv, tq, tdo, a) != cudaSuccess) return -1;
+  PG_CHECK_LAUNCH("attention_bwd");
+  return 0;
+}
+
+// dq_acc: fp32 workspace [B*S, H*D]; delta: fp32 [B, H, S]
+extern "C" int pg_attention_bwd(const void* qkv, const float* slopes, const void* out, const float* lse,
+                                const void* dout, void* dqkv, float* dq_acc, float* delta, int B, int S, int H,
+                                int D, float softmax_scale, cudaStream_t s) {
+  if (D != 64 && D != 128) return -1;
+  const int64_t rows = static_cast<int64_t>(B) * S;
+  CUtensorMap tkv, tq, tdo;
+  if (att_tmap(&tkv, qkv, rows, static_cast<uint64_t>(H) * 3 * D, ATT_BN) != 0) return -1;
+  if (att_tmap(&tq, qkv, rows, static_cast<uint64_t>(H) * 3 * D, ATT_BWD_BM) != 0) return -1;
+  if (att_tmap(&tdo, dout, rows, static_cast<uint64_t>(H) * D, ATT_BWD_BM) != 0) return -1;
+  if (cudaMemsetAsync(dq_acc, 0, rows * H * D * sizeof(float), s) != cudaSuccess) return -1;
+  {
+    if (launch_pdl(attention_delta_kernel, dim3((unsigned)((rows * 32 + 255) / 256)), dim3(256), 0, s,
+                   (const __nv_bfloat16*)dout, (const __nv_bfloat16*)out, delta, B, S, H, D) != cudaSuccess) return -1;
+    PG_CHECK_LAUNCH("attention_delta");
+  }
+  AttBwdArgs a;
+  a.lse = lse; a.delta = delta; a.slopes = slopes; a.dq_acc = dq_acc;
+  a.dqkv = (__nv_bfloat16*)dqkv;
+  a.B = B; a.S = S; a.H = H;
+  a.scale = softmax_scale > 0.f ? softmax_scale : 1.0f / sqrtf(static_cast<float>(D));
+  a.scale_log2 = a.scale * kLog2e;
+  const int rc = D == 64 ? launch_att_bwd<64>(tkv, tq, tdo, a, s) : launch_att_bwd<128>(tkv, tq, tdo, a, s);
+  if (rc != 0) return rc;
+  const int64_t total = rows * H * D;
+  if (launch_pdl(attention_dq_convert_kernel, dim3((unsigned)((total / 8 + 255) / 256)), dim3(256), 0, s, (const float*)dq_acc,
+                 (__nv_bfloat16*)dqkv, (int64_t)rows, H, D) != cudaSuccess) return -1;
+  PG_CHECK_LAUNCH("attention_dq_convert");
+  return 0;
+}

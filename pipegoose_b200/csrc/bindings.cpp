@@ -115,7 +115,6 @@ void gemm(const torch::Tensor& a, const torch::Tensor& b, torch::Tensor out, boo
     parse_grad_rs(ag["grad_rs"].cast<py::dict>(), &d.grad_rs);
   }
   if (ag.contains("k_splits")) d.k_splits = ag["k_splits"].cast<int>();
-  if (ag.contains("cta_pair")) d.cta_pair = ag["cta_pair"].cast<int>();
   if (ag.contains("n_comm")) {
     d.n_comm = ag["n_comm"].cast<int>();
     d.ag_dst = reinterpret_cast<void*>(ag["dst"].cast<int64_t>());
@@ -468,7 +467,7 @@ void barrier_peers(std::vector<int64_t> peer_flags, int64_t rank, int64_t epoch)
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.def("gemm", &gemm, "tcgen05 bf16 GEMM with fused epilogue / chunked collectives",
+  m.def("gemm", &gemm, "wgmma bf16 GEMM with fused epilogue / chunked collectives",
         py::arg("a"), py::arg("b"), py::arg("out"), py::arg("a_mn") = false, py::arg("b_mn") = false,
         py::arg("bias") = py::none(), py::arg("residual") = py::none(), py::arg("aux") = py::none(),
         py::arg("flags") = 0, py::arg("block_n") = 0, py::arg("max_ctas") = 0,

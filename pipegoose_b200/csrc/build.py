@@ -1,7 +1,7 @@
-"""In-tree build of the sm_100a extension ``pipegoose_b200/_C*.so``.
+"""In-tree build of the sm_90a extension ``pipegoose_b200/_C*.so``.
 
 Every ``*.cu`` under ``csrc/`` is compiled straight by nvcc with
-``-gencode arch=compute_100a,code=sm_100a -lineinfo`` (no torch headers, so a kernel file
+``-gencode arch=compute_90a,code=sm_90a -lineinfo`` (no torch headers, so a kernel file
 rebuilds in seconds); ``bindings.cpp`` is the only translation unit that sees torch.  Objects
 are cached under ``csrc/build/`` keyed by a content hash of the source and the headers.
 """
@@ -19,7 +19,7 @@ CSRC = Path(__file__).resolve().parent
 PKG = CSRC.parent
 BUILD = CSRC / "build"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH_FLAGS + [
     "-O3", "-std=c++17", "-lineinfo", "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC", "-Xptxas", "-v",
@@ -27,7 +27,7 @@ NVCC_FLAGS = ARCH_FLAGS + [
 
 
 # PIPEGOOSE_B200_BUILD_VARIANT=<name> + PIPEGOOSE_B200_NVCC_EXTRA="-DFOO=1 ...": build pipegoose_b200/_C_<name>.so with extra
-# nvcc flags next to the main extension (loaded with PIPEGOOSE_B200_EXT=<name>): A/B of kernel variants in ONE gpurun call
+# nvcc flags next to the main extension (loaded with PIPEGOOSE_B200_EXT=<name>): A/B of kernel variants in one process
 VARIANT = os.environ.get("PIPEGOOSE_B200_BUILD_VARIANT", "")
 NVCC_FLAGS = NVCC_FLAGS + os.environ.get("PIPEGOOSE_B200_NVCC_EXTRA", "").split()
 if VARIANT:

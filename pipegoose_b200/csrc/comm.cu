@@ -215,9 +215,9 @@ __global__ void __launch_bounds__(512) allreduce_f32_kernel(PeerPtrs p, float* _
   allreduce_f32_body<8>(p, mc, world, rank, offset, n, bucket_elems, scale, rs_only, epoch, grid_ctr);
 }
 
-// Co-resident form: 128 threads x <= 64 registers and a few bytes of shared memory — small enough to be scheduled on an
-// SM that a persistent GEMM CTA occupies (the GEMM launches with 384 x 128 registers and ~210 KB of shared memory, see
-// gemm_sm100.cuh), so the bucket reduction really runs WHILE backward computes instead of at kernel boundaries.
+// Small form: 128 threads x <= 64 registers and a few bytes of shared memory.  A persistent GEMM CTA holds its SM's
+// whole register file (see gemm_sm90.cuh), so neither form runs next to a GEMM CTA: while backward computes, the
+// GEMM grids are capped (pg_set_gemm_cta_cap, ops/comm.py) to leave the reducer's SMs free.
 // 2 CTAs per SM x 128 threads x 4 x 16 B = 16 KB in flight per SM (2.4 MB over the chip: the NVLink bandwidth-delay product)
 __global__ void __launch_bounds__(128, 8) /* <= 64 registers per thread */
     allreduce_f32_small_kernel(PeerPtrs p, float* __restrict__ mc, int world, int rank, int64_t offset, int64_t n,
@@ -374,7 +374,7 @@ extern "C" int pg_rs_reduce(const void* staging, int num_src, int64_t src_stride
   if (cols % 8 != 0) return -1;
   const int64_t nvec = static_cast<int64_t>(rows) * cols / 8;
   int blocks = static_cast<int>((nvec + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   rs_reduce_kernel<<<blocks, 256, 0, s>>>((const __nv_bfloat16*)staging, num_src, src_stride_elems,
                                           arrive_ctr, expected, (const __nv_bfloat16*)bias,
                                           (const __nv_bfloat16*)residual, (__nv_bfloat16*)out, rows, cols);
@@ -397,7 +397,7 @@ extern "C" int pg_allreduce_f32(float* const* peer_bufs, float* mc_buf, int worl
   }
   // overlapped with backward: a handful of CTAs on the SMs the persistent GEMMs leave free (pg_set_gemm_cta_cap);
   // after backward (nothing else runs): enough CTAs to keep ~3 MB in flight over NVLink
-  if (blocks < 0) {  // co-resident form: -blocks small CTAs that fit next to the persistent GEMM CTAs
+  if (blocks < 0) {  // small form: -blocks CTAs of 128 threads
     allreduce_f32_small_kernel<<<-blocks, 128, 0, s>>>(p, mc_buf, world, rank, offset_elems, n, bucket_elems, scale,
                                                        reduce_scatter_only, epoch, peer_flags[rank] + 2 * PG_MAX_PEERS);
     PG_CHECK_LAUNCH("allreduce_f32_small");
@@ -455,7 +455,7 @@ extern "C" int pg_rs_reduce_mc(const void* mc_partial, const uint32_t* arrive_ct
   if (cols % 8 != 0) return -1;
   const int64_t nvec = static_cast<int64_t>(rows) * cols / 8;
   int blocks = static_cast<int>((nvec + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   rs_reduce_mc_kernel<<<blocks, 256, 0, s>>>((const __nv_bfloat16*)mc_partial, arrive_ctr, num_src, expected,
                                              (const __nv_bfloat16*)bias, (const __nv_bfloat16*)residual,
                                              (__nv_bfloat16*)out, rows, cols);

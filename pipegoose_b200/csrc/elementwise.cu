@@ -595,7 +595,7 @@ extern "C" int pg_layernorm_bwd(const void* dy, const void* x, const void* gamma
   PG_CHECK_LAUNCH("layernorm_bwd_dx");
   if (dgamma != nullptr) {
     const int cb = (h + 255) / 256;
-    int rsplit = (148 * 4 + cb - 1) / cb;
+    int rsplit = (132 * 4 + cb - 1) / cb;
     if (rsplit > (rows + 63) / 64) rsplit = (rows + 63) / 64;
     if (rsplit < 1) rsplit = 1;
     const int rpb = (rows + rsplit - 1) / rsplit;
@@ -609,7 +609,7 @@ extern "C" int pg_layernorm_bwd(const void* dy, const void* x, const void* gamma
 extern "C" int pg_colsum(const void* x, int ld, float* out, int rows, int cols, cudaStream_t s) {
   if (rows == 0 || cols == 0) return 0;
   const int cb = (cols + 255) / 256;
-  int rsplit = (148 * 4 + cb - 1) / cb;
+  int rsplit = (132 * 4 + cb - 1) / cb;
   if (rsplit > (rows + 63) / 64) rsplit = (rows + 63) / 64;
   if (rsplit < 1) rsplit = 1;
   const int rpb = (rows + rsplit - 1) / rsplit;

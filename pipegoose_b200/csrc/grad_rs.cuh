@@ -7,11 +7,19 @@
 
 namespace pg {
 
+// owner slice of element `off` (relative to g.start), clamped to [0, world): compares instead of a 64-bit division,
+// which compiles to a subroutine call
+PG_DEVICE int grs_owner(const PgGradRS& g, long long off) {
+  int k = 0;
+#pragma unroll
+  for (int i = 1; i < PG_MAX_PEERS; ++i)
+    if (i < g.world && off >= i * g.seg) k = i;
+  return k;
+}
+
 PG_DEVICE float* grs_target(const PgGradRS& g, const float* local_ptr) {
   const long long off = local_ptr - g.local;
-  long long k = (off - g.start) / g.seg;
-  k = k < 0 ? 0 : (k >= g.world ? g.world - 1 : k);
-  return g.peer[static_cast<int>(k)] + off;
+  return g.peer[grs_owner(g, off - g.start)] + off;
 }
 
 PG_DEVICE void grs_add4_at(const PgGradRS& g, float* target, float4 v) {

@@ -40,7 +40,6 @@ typedef struct PgGemmDesc {
   int flags;  // EpiFlags
   int block_n;   // 0 = auto
   int k_splits;  // 0 = auto (fp32 outputs only), 1 = never split, >1 = forced
-  int cta_pair;  // 0 = auto, -1 = 1-CTA tiles only, 1 = CTA-pair (cta_group::2, 256-row) tiles
   int max_ctas;  // 0 = all SMs
   int num_chunks, chunk_rows, first_chunk;
   const uint32_t* chunk_flags;
@@ -74,7 +73,7 @@ typedef struct PgGemmDesc {
   int ce_valid;
 } PgGemmDesc;
 
-// ---- attention_sm100.cu
+// ---- attention_sm90.cu
 int pg_attention_fwd(const void* qkv, const float* slopes, void* out, float* lse, int B, int S, int H, int D,
                      float softmax_scale, cudaStream_t s);
 int pg_attention_bwd(const void* qkv, const float* slopes, const void* out, const float* lse, const void* dout,

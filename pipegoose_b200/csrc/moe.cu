@@ -9,7 +9,7 @@
 //                 (k*n + token) and the gate weight; the owner's per-expert arrival counters are
 //                 bumped with a system-scope release so the expert GEMM (chunk = expert) can start on
 //                 an expert as soon as all sources finished pushing.
-// Combine is the epilogue of the last expert GEMM (EPI_SCATTER in gemm_sm100.cuh): each output row is
+// Combine is the epilogue of the last expert GEMM (EPI_SCATTER in gemm_sm90.cuh): each output row is
 // scaled by its gate weight and stored into the source rank's combine buffer at the return address.
 #include "launch.h"
 #include "ptx.cuh"
@@ -192,7 +192,7 @@ extern "C" int pg_moe_route(const void* x, const void* wg, const void* bg, const
     set = true;
   }
   int blocks = (n + 7) / 8;
-  if (blocks > 148 * 2) blocks = 148 * 2;
+  if (blocks > 132 * 2) blocks = 132 * 2;
   moe_route_kernel<<<blocks, 256, smem, s>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)wg,
                                              (const __nv_bfloat16*)bg, jitter, n, h, E, top_k, capacity, probs,
                                              topk_idx, topk_prob, pos, counts, prob_sum, zsum, lse_out);

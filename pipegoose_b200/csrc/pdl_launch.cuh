@@ -2,7 +2,6 @@
 //   default / PIPEGOOSE_B200_PDL=1 : kernels are launched with cudaLaunchAttributeProgrammaticStreamSerialization, so a
 //                          kernel's prologue overlaps the tail of its predecessor (every kernel launched through here
 //                          calls pdl_launch_dependents() at its start and pdl_wait() before its first dependent access).
-//                          Measured on B200 (bloom-560m step, 1 GPU, same box): 42.91 -> 42.52 ms.
 //   PIPEGOOSE_B200_PDL=0 : plain stream-ordered launches (the griddepcontrol instructions are no-ops)
 #pragma once
 #include <cuda_runtime.h>

@@ -1,7 +1,8 @@
-// Thin inline-PTX wrappers for the sm_100a primitives used by every kernel in this
-// tree: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld),
-// system-scope acquire/release flag traffic for cross-GPU protocols, and vector
-// global loads/stores.  No CUTLASS dependency: the bit layouts follow the PTX ISA.
+// Thin inline-PTX wrappers for the sm_90a primitives used by every kernel in this
+// tree: mbarrier, TMA (cp.async.bulk.tensor), named barriers, system-scope
+// acquire/release flag traffic for cross-GPU protocols, and vector global
+// loads/stores (wgmma lives in wgmma.cuh).  No CUTLASS dependency: the bit layouts
+// follow the PTX ISA.
 #pragma once
 #include <cstdio>
 #include <cuda.h>
@@ -128,183 +129,9 @@ PG_DEVICE void bulk_store_1d(void* gdst, const void* smem_src, uint32_t bytes) {
                : "memory");
 }
 
-// ----------------------------------------------------------------------------------
-// tcgen05 / TMEM
-// ----------------------------------------------------------------------------------
-PG_DEVICE void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-PG_DEVICE void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-PG_DEVICE void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-PG_DEVICE void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-PG_DEVICE void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (bf16/fp16 inputs, fp32 accumulate).
-PG_DEVICE void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A operand from TMEM (TS form): D[tmem] (+)= A[tmem] * B[smem desc].
-PG_DEVICE void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread retire.
-PG_DEVICE void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-// ---- CTA-pair (cta_group::2) forms: the two CTAs of a cluster on one TPC share one MMA ----
-PG_DEVICE uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-PG_DEVICE void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same smem location in CTA `rank` of the cluster
-PG_DEVICE uint32_t mapa_shared(uint32_t saddr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
-}
-PG_DEVICE void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load into this CTA's smem whose completion bytes are counted on a barrier of the pair's leader CTA
-PG_DEVICE void tma_load_2d_cta2(void* smem_dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int32_t c0,
-                                int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-PG_DEVICE void tmem_alloc_cta2(uint32_t* smem_result, uint32_t ncols) {  // one warp in EACH CTA of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-PG_DEVICE void tmem_relinquish_cta2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-PG_DEVICE void tmem_dealloc_cta2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-// D[tmem of both CTAs] (+)= A[256 rows: 128 from each CTA's smem] * B[N: N/2 from each CTA's smem]
-PG_DEVICE void umma_f16_cta2(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on the barrier at the same smem offset in every CTA of `cta_mask` once prior MMAs retire
-PG_DEVICE void umma_commit_cta2(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
-PG_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-PG_DEVICE void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive 32-bit columns: thread t of the warp receives columns
-// [col, col+32) of TMEM lane (lane_base + t).
-PG_DEVICE void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]),
-        "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]),
-        "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-PG_DEVICE void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-PG_DEVICE void tmem_st_32x16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-      "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]),
-      "r"(v[15])
-      : "memory");
-}
-
-// Shared-memory matrix descriptor (tcgen05 flavour: version=1 at bits [46,48)).
-//   start address  bits [0,14)   (byte address >> 4)
-//   leading offset bits [16,30)  (bytes >> 4)
-//   stride offset  bits [32,46)  (bytes >> 4)
-//   layout type    bits [61,64)  (2 = 128-byte swizzle)
-PG_DEVICE uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
-// Instruction descriptor for kind::f16 with BF16 inputs and FP32 accumulation.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, bool a_mn_major,
-                                                       bool b_mn_major) {
-  return (1u << 4)                                  // D format: F32
-         | (1u << 7)                                // A format: BF16
-         | (1u << 10)                               // B format: BF16
-         | (static_cast<uint32_t>(a_mn_major) << 15)  // A major
-         | (static_cast<uint32_t>(b_mn_major) << 16)  // B major
-         | (static_cast<uint32_t>(N >> 3) << 17)    // N / 8
-         | (static_cast<uint32_t>(M >> 4) << 24);   // M / 16
+// named barrier over `count` threads (a multiple of 32) of the CTA; id 0 is __syncthreads
+PG_DEVICE void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // ----------------------------------------------------------------------------------
@@ -359,6 +186,16 @@ PG_DEVICE void spin_until_ge(const uint32_t* p, uint32_t want, int site) {
     }
   }
 }
+// The same wait without the diagnostic printf, for kernels that issue wgmma: a printf (an ABI call) anywhere in such a
+// kernel makes ptxas serialise every wgmma of it (C7510), even when the call sits in another warp role.  A flag that
+// never arrives still traps after the budget: the host sees a launch failure instead of a wedged GPU, without the site.
+PG_DEVICE void spin_until_ge_quiet(const uint32_t* p, uint32_t want) {
+  if (ld_acquire_sys(p) >= want) return;
+  const long long t0 = clock64();
+  while (ld_acquire_sys(p) < want) {
+    if (clock64() - t0 > PG_SPIN_BUDGET_CYCLES) __trap();
+  }
+}
 // generic-proxy writes (peer flags / data) -> later async-proxy (TMA) reads of global memory
 PG_DEVICE void fence_proxy_async_global() {
   asm volatile("fence.proxy.async.global;" ::: "memory");
@@ -366,7 +203,7 @@ PG_DEVICE void fence_proxy_async_global() {
 
 // ----------------------------------------------------------------------------------
 // programmatic dependent launch (PDL): the next kernel of the stream may start its prologue (smem carve-up,
-// barrier init, TMEM allocation, tensor-map prefetch) while this one is still running; it blocks in pdl_wait()
+// barrier init, tensor-map prefetch) while this one is still running; it blocks in pdl_wait()
 // until every predecessor has completed and its memory operations are visible.  Both are no-ops for kernels
 // that were not launched with the programmatic-stream-serialization attribute.
 // ----------------------------------------------------------------------------------

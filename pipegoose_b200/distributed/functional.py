@@ -3,7 +3,7 @@ distributed/functional.py:30-182).  Every function is a no-op for a group of one
 
 These are the *library* collectives (NCCL / gloo through torch.distributed): they are the
 plumbing and the always-correct fallback.  The hot paths of the parallel wrappers use the fused
-sm_100a kernels in ``pipegoose_b200.ops`` instead and only fall back to these on CPU/gloo.
+sm_90a kernels in ``pipegoose_b200.ops`` instead and only fall back to these on CPU/gloo.
 ``reduce_scatter`` and ``all_to_all`` exist here (the reference left the former as a stub and has
 no all-to-all at all).
 """

@@ -1,4 +1,4 @@
-"""B200-native Bloom (``BloomForCausalLM``) with the same module tree and parameter names as
+"""H100-native Bloom (``BloomForCausalLM``) with the same module tree and parameter names as
 🤗 transformers' Bloom, so HF state dicts load unchanged and the name-based parallel mappings
 (reference nn/tensor_parallel/parallel_mapping.py:4-52) apply to both.
 

@@ -1,4 +1,4 @@
-"""GPT-2 on the same sm_100a sub-layer kernels as Bloom — the second model family of the reference's tests
+"""GPT-2 on the same sm_90a sub-layer kernels as Bloom — the second model family of the reference's tests
 (tests/nn/pipeline_parallel/test_partitioner.py runs its partitioner on 🤗 ``gpt2``).
 
 A GPT-2 block is a Bloom block without ALiBi: pre-LayerNorm, fused QKV, causal softmax(QK^T/sqrt(D))V, output

@@ -57,7 +57,7 @@ class ExpertParallel(Parallel):
                 continue
             expert = self.expert if self.expert is not None else block.mlp
             if self._use_fused(expert):
-                # NVLink all-to-all dispatch/combine + grouped tcgen05 expert GEMMs (ops/moe.py)
+                # NVLink all-to-all dispatch/combine + grouped wgmma expert GEMMs (ops/moe.py)
                 from pipegoose_b200.ops.moe import FusedExpertLayer
 
                 block.mlp = FusedExpertLayer(self.num_experts, expert, self.router, self.parallel_context)

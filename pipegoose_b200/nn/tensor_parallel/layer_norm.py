@@ -1,6 +1,6 @@
 """LayerNorm under tensor parallelism (parity: reference nn/tensor_parallel/layer_norm.py:8-25): parameters are
 replicated, nothing is communicated.  It is ``torch.nn.LayerNorm`` plus a fast path — CUDA bf16 rows go through the fused
-sm_100a LayerNorm kernel (ops/kernels.py) — which also makes the class swap of ``TensorParallel`` a plain
+sm_90a LayerNorm kernel (ops/kernels.py) — which also makes the class swap of ``TensorParallel`` a plain
 subclass swap that ``deparallelize()`` can undo."""
 from __future__ import annotations
 

@@ -3,7 +3,7 @@ reference nn/tensor_parallel/linear.py:17-82): a column-parallel layer owns a bl
 all-gathers them), a row-parallel layer owns a block of input features and all-reduces its partial products.
 
 Both are one class body: what differs is the weight dimension that is split (``shard_dim``) and the pair of
-communication ops around the local GEMM, which runs on the tcgen05 kernel with the bias in its epilogue
+communication ops around the local GEMM, which runs on the wgmma kernel with the bias in its epilogue
 (``ops.functional.linear``).  The sequence-parallel fast path with fused all-gather→GEMM / GEMM→reduce-scatter kernels
 lives in ``pipegoose_b200.models`` / ``ops/functional.py``; these layers exist so that any 🤗 model can be sharded.
 """

@@ -1,4 +1,4 @@
-"""Python front-end of the sm_100a kernels.
+"""Python front-end of the sm_90a kernels.
 
 ``native()`` returns the in-tree extension module (``pipegoose_b200/_C.so``, built by
 ``pipegoose_b200/csrc/build.py``).  On a machine with a CUDA device the extension is mandatory:
@@ -105,7 +105,7 @@ def has_kernel(name: str) -> bool:
 
 
 def use_native(*tensors) -> bool:
-    """True when the op must run on the sm_100a kernels (CUDA bf16 inputs).
+    """True when the op must run on the sm_90a kernels (CUDA bf16 inputs).
 
     Raises if CUDA tensors are given but the extension is missing: a GPU run never degrades to
     an eager fallback silently.

@@ -4,8 +4,8 @@
 ``query_key_value`` produces), the result is ``[B*S, n_head*D]``.  Scores are
 ``q.k / sqrt(D) + slope[head] * key_position`` under a causal mask, softmax in fp32.
 
-Two implementations share this contract: the sm_100a flash kernel (``csrc/attention_sm100.cu``:
-tcgen05 QK^T / PV with TMEM accumulators, online softmax, never materialising ``[S, S]``) and
+Two implementations share this contract: the sm_90a flash kernel (``csrc/attention_sm90.cu``:
+wgmma QK^T / PV with register accumulators, online softmax, never materialising ``[S, S]``) and
 the PyTorch reference below (CPU tests, numerics oracle).
 """
 from __future__ import annotations
@@ -104,7 +104,7 @@ def unpad_heads(x: torch.Tensor, n_head: int, parts: int, D: int, DP: int) -> to
 
 
 class _AlibiAttentionPadded(torch.autograd.Function):
-    """Head sizes the tcgen05 kernel has no tile shape for (e.g. D=80, bloom-3b): the heads are zero-padded to the
+    """Head sizes the wgmma kernel has no tile shape for (e.g. D=80, bloom-3b): the heads are zero-padded to the
     next supported width and run through the same flash kernel with the softmax scale of the TRUE width — padded q/k
     columns add nothing to the scores, padded v columns produce output columns that are sliced away."""
 

@@ -2,7 +2,7 @@
 
 ``FusedTPEngine`` drives the two tensor-parallel kernels
 
-* **all-gather -> GEMM** (`ag_gemm`, `ag_gemm_nn`): ONE launch of the tcgen05 GEMM kernel in which
+* **all-gather -> GEMM** (`ag_gemm`, `ag_gemm_nn`): ONE launch of the wgmma GEMM kernel in which
   a few communication CTAs pull every peer's activation shard through NVSwitch with bulk async
   copies into the local gathered operand while the remaining CTAs run the MMA tiles, visiting the
   row chunks in arrival order (local shard first) and acquiring a per-chunk counter before the
@@ -28,37 +28,24 @@ _BM = 128
 import os
 
 N_COMM_CTAS = int(os.environ.get("PIPEGOOSE_B200_NCOMM", "16"))
-# 1: GEMM -> reduce-scatter reduces the local chunk in its own epilogue (no reduce kernel; measured 10 us slower per
-# op at T=2 because the staged partials are read without prefetch); 0 (default): separate rs_reduce kernel
+# 1: GEMM -> reduce-scatter reduces the local chunk in its own epilogue (no reduce kernel, but the staged partials are
+# read without prefetch); 0 (default): separate rs_reduce kernel
 RS_FUSED_REDUCE = os.environ.get("PIPEGOOSE_B200_RS_FUSED_REDUCE", "0") == "1"
 
 
-RS_PAIR = os.environ.get("PIPEGOOSE_B200_RS_PAIR", "auto")  # CTA pairs in GEMM -> reduce-scatter: auto / 0 / 1
-
-
-def pick_tiling(rows: int, n: int, k: int, chunks: int, ctas: int, b_mn: bool, pair_mode: str = "auto"):
-    """``(block_n, cta_pair)`` for a GEMM -> reduce-scatter: mirror of ``pick_bn`` in csrc/gemm_sm100.cu (the
-    arrival counters of a reduce-scatter are counted in tiles, so both sides must agree on the tiling).
-    CTA pairs (tcgen05 ``cta_group::2``, 256-row tiles) where the operand feed is the limit: long K or many tiles."""
-    tiles1 = ((rows + _BM - 1) // _BM) * ((n + 255) // 256) * chunks
-    pair = rows % (2 * _BM) == 0 and ctas >= 2 and (k >= 2048 or tiles1 >= 3 * ctas)
-    if pair_mode in ("0", "1"):
-        pair = pair_mode == "1" and rows % (2 * _BM) == 0 and ctas >= 2
-    bm = 2 * _BM if pair else _BM
-    units = ctas // 2 if pair else ctas
-    cands = ((256, 1.0), (192, 0.80), (128, 0.70)) if pair else ((256, 1.0), (192, 0.93), (128, 0.82), (64, 0.55))
+def pick_tiling(rows: int, n: int, k: int, chunks: int, ctas: int) -> int:
+    """``block_n`` for a GEMM -> reduce-scatter: mirror of ``pick_bn`` in csrc/gemm_sm90.cu (the arrival counters of a
+    reduce-scatter are counted in tiles, so both sides must agree on the tiling)."""
     best, best_cost = 256, float("inf")
-    for bn, eff in cands:
-        if pair and b_mn and (bn // 2) % 64 != 0:
-            continue
+    for bn, eff in ((256, 1.0), (192, 0.93), (128, 0.82), (64, 0.55)):
         if bn > 64 and n <= bn // 2:
             continue
-        tiles = ((rows + bm - 1) // bm) * ((n + bn - 1) // bn) * chunks
-        waves = (tiles + units - 1) // units
+        tiles = ((rows + _BM - 1) // _BM) * ((n + bn - 1) // bn) * chunks
+        waves = (tiles + ctas - 1) // ctas
         cost = waves * bn / eff
         if cost < best_cost * 0.97:
             best, best_cost = bn, cost
-    return best, pair
+    return best
 
 
 class FusedTPEngine:
@@ -183,8 +170,8 @@ class FusedTPEngine:
         self.rs_calls += 1
         slot = self.rs_calls & 1
         k = a.shape[1]
-        bn, pair = pick_tiling(m_local, n, k, T, self.num_sms, b_mn, RS_PAIR)
-        # every CTA bumps the owner's counter once per tile it stored (both CTAs of a pair do)
+        bn = pick_tiling(m_local, n, k, T, self.num_sms)
+        # every CTA bumps the owner's counter once per tile it stored
         tiles_per_chunk = ((m_local + _BM - 1) // _BM) * ((n + bn - 1) // bn)
         self.rs_expected += tiles_per_chunk
         src_stride = m_local * n  # elements between two sources' slots
@@ -193,14 +180,14 @@ class FusedTPEngine:
         out = torch.empty(m_local, n, dtype=torch.bfloat16, device=a.device)
         if RS_FUSED_REDUCE:
             # the epilogue of this rank's own (last visited) chunk adds the peers' staged partials + bias + residual
-            ag = {"cta_pair": 1 if pair else -1, "rank": r, "rs_wait": ws.sig_ptr(r, S.SIG_RS_ARRIVE),
+            ag = {"rank": r, "rs_wait": ws.sig_ptr(r, S.SIG_RS_ARRIVE),
                   "rs_wait_value": self.rs_expected,
                   "rs_in": [ws.data_ptr(r, self._rs_off(slot) + s * src_stride * 2) for s in range(T)]}
             native().gemm(a, weight, out, False, b_mn, bias, residual, None, 0, bn, 0,
                           T, (r + 1) % T, 0, 0, out_peer, arrive, ag)
             return out
         native().gemm(a, weight, self._dummy_out(n, a.device), False, b_mn, None, None, None, 0, bn, 0,
-                      T, (r + 1) % T, 0, 0, out_peer, arrive, {"cta_pair": 1 if pair else -1})
+                      T, (r + 1) % T, 0, 0, out_peer, arrive, {})
         native().rs_reduce(ws.data_ptr(r, self._rs_off(slot)), T, src_stride, ws.sig_ptr(r, S.SIG_RS_ARRIVE),
                            self.rs_expected, bias, residual, out)
         return out
@@ -353,16 +340,14 @@ class FusedDPEngine:
         return param, grad
 
     # NVLS (multimem.ld_reduce / multimem.st through the NVSwitch multicast object): "auto" = groups of >= 4 ranks.
-    # Measured on 2 x B200 (dp=2, bloom-560m, profiles/validate_2gpu_r2.log): 45.76 ms/step with NVLS vs 45.14 without —
-    # with ONE peer the switch-side reduction saves no bytes and adds latency; from 4 ranks on a pull through the switch
+    # With ONE peer the switch-side reduction saves no bytes and adds latency; from 4 ranks on a pull through the switch
     # moves 1/world of the bytes of a pull from every peer.
     NVLS_REDUCE = os.environ.get("PIPEGOOSE_B200_NVLS_REDUCE", "auto")
     NVLS_ALLGATHER = os.environ.get("PIPEGOOSE_B200_NVLS_ALLGATHER", "auto")
     # 1: reduce-scatter the matrices' gradients inside the kernels that produce them (red.global.add into the owner's
-    # buffer).  OFF by default — measured on 2 x B200 (dp=2, bloom-560m): 69.7 ms/step against 45.8 ms with the bucketed
-    # reducer (numerically identical, max rel. loss difference 4.5e-6): NVLink executes remote atomics at ~2.5-3 G
-    # operations/s whatever their width (v4.f32: ~46 GB/s; four scalar reds: 157 ms/step), far below the 750 GB/s that
-    # plain peer loads / stores reach, and the wgrad epilogues stall on them.  Kept as an option and as a tested kernel path.
+    # buffer).  OFF by default: NVLink remote atomics run far below the bandwidth of plain peer loads / stores and the
+    # wgrad epilogues stall on them (the earlier sm_100a build measured it slower than the bucketed reducer; not
+    # re-measured on H100).  Kept as an option and as a tested kernel path.
     INLINE_RS = os.environ.get("PIPEGOOSE_B200_DP_INLINE_RS", "0") == "1"
     # 1: four scalar red.global.add.f32 per 16 bytes instead of one red.global.add.v4.f32 (diagnosis)
     INLINE_SCALAR_RED = os.environ.get("PIPEGOOSE_B200_DP_INLINE_SCALAR", "0") == "1"
@@ -418,21 +403,25 @@ class FusedDPEngine:
     def _flag_ptrs(self):
         return [self.ws.sig_ptr(p, S.SIG_BARRIER) for p in range(self.world)]
 
-    # CTAs of a gradient reduction that overlaps backward / runs after it (nothing else runs then: NVLink-bound)
-    # negative: that many CTAs of the CO-RESIDENT form (128 threads, 62 registers: fits next to a persistent GEMM CTA,
-    # see csrc/comm.cu); positive: 512-thread CTAs that only get SMs at GEMM kernel boundaries (round 1).  Measured on
-    # 2 x B200 at dp = 2 (profiles/ab_2gpu_r2.log): 64 / 96 big CTAs 45.57 ms, -296 / -592 small CTAs 44.64 ms per step.
-    OVERLAP_CTAS = int(os.environ.get("PIPEGOOSE_B200_DP_OVERLAP_CTAS", "-296"))
-    TAIL_CTAS = int(os.environ.get("PIPEGOOSE_B200_DP_TAIL_CTAS", "-592"))
-    # 1: persistent GEMM grids leave OVERLAP_CTAS SMs free while reductions overlap backward
-    CAP_GEMMS = os.environ.get("PIPEGOOSE_B200_DP_CAP_GEMMS", "0") == "1"
+    # CTAs of a gradient reduction that overlaps backward / runs after it.  Positive: 512-thread CTAs; negative: that many
+    # CTAs of the small form (128 threads, <= 64 registers, see csrc/comm.cu).  A persistent GEMM CTA holds its SM's whole
+    # register file, so while reductions overlap backward the GEMM grids are capped to leave |OVERLAP_CTAS| SMs to the
+    # reducer (CAP_GEMMS): a reducer CTA, which waits on peers inside the kernel, then never keeps a GEMM CTA from
+    # becoming resident.  The tail reductions run after the last backward kernel, and finalize() orders the compute
+    # stream after them, so no GEMM runs next to them.  16 CTAs keep ~1 MB in flight over NVLink (8 x 16 B loads per
+    # thread), about the bandwidth-delay product of one NVLink4 direction; the tail uses 48 (one per ~3 SMs of 132).
+    OVERLAP_CTAS = int(os.environ.get("PIPEGOOSE_B200_DP_OVERLAP_CTAS", "16"))
+    TAIL_CTAS = int(os.environ.get("PIPEGOOSE_B200_DP_TAIL_CTAS", "48"))
+    # 0: GEMM grids keep every SM while reductions overlap backward; the reducer then depends on GEMM kernel boundaries
+    # to become resident, and a tensor-parallel GEMM that waits on a peer can stall it — only for experiments
+    CAP_GEMMS = os.environ.get("PIPEGOOSE_B200_DP_CAP_GEMMS", "1") == "1"
 
     def begin_overlap(self):
-        """Backward starts reducing buckets: persistent GEMM grids leave ``OVERLAP_CTAS`` SMs to the reducer
-        (a persistent GEMM whose CTAs cannot all be resident stalls behind the reducer's CTAs)."""
+        """Backward starts reducing buckets: persistent GEMM grids leave ``|OVERLAP_CTAS|`` SMs to the reducer (a
+        reducer CTA occupies at most one SM; a persistent GEMM whose CTAs cannot all be resident stalls behind it)."""
         if self.CAP_GEMMS and not getattr(self, "_capped", False):
             sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-            native().set_gemm_cta_cap((sms - self.OVERLAP_CTAS) // 2 * 2)
+            native().set_gemm_cta_cap(max(1, sms - abs(self.OVERLAP_CTAS)))
             self._capped = True
 
     def end_overlap(self):

@@ -23,16 +23,14 @@ from pipegoose_b200.ops import kernels as K
 
 # lm_head under tensor parallelism through the fused all-gather->GEMM / GEMM->reduce-scatter kernels instead of NCCL
 # around a plain GEMM, and LayerNorm backward writing dx straight into the staging slot of the next backward all-gather.
-# Validated on 2 x B200 (tests/test_gpu_multi.py::test_tp2_bloom_matches_single_gpu passes with both; bloom-560m TP2 step
-# 45.89 -> 45.28 ms, profiles/validate_2gpu_r2.log); PIPEGOOSE_B200_FUSED_LM_HEAD=0 / _LNBWD_TO_STAGE=0 switch them off.
+# Covered by tests/test_gpu_multi.py::test_tp2_bloom_matches_single_gpu (2 GPUs) with both;
+# PIPEGOOSE_B200_FUSED_LM_HEAD=0 / _LNBWD_TO_STAGE=0 switch them off.
 import os as _os
 
 _FUSED_LM_HEAD = _os.environ.get("PIPEGOOSE_B200_FUSED_LM_HEAD", "1") == "1"
 _LNBWD_TO_STAGE = _os.environ.get("PIPEGOOSE_B200_LNBWD_TO_STAGE", "1") == "1"
-# cross-entropy statistics from the lm_head GEMM's epilogue instead of a pass over the logits.  Measured on a B200
-# (profiles/ncu_lm_head_ce_epilogue_r2.txt, profiles/validate_1gpu_r2.log): the 8192 x 125440 x 1024 logits GEMM takes
-# 1.93 ms with the partials in its epilogue against 1.70 ms without, and the 0.74 ms statistics pass over the logits is
-# gone; the bloom-560m step reports the same loss.  PIPEGOOSE_B200_CE_IN_EPILOGUE=0 restores the separate pass.
+# cross-entropy statistics from the lm_head GEMM's epilogue instead of a pass over the logits: the statistics pass
+# never re-reads the [tokens, vocab] logits.  PIPEGOOSE_B200_CE_IN_EPILOGUE=0 restores the separate pass.
 _CE_IN_EPILOGUE = _os.environ.get("PIPEGOOSE_B200_CE_IN_EPILOGUE", "1") == "1"
 
 
@@ -195,7 +193,7 @@ class LinearResidual(torch.autograd.Function):
 
 class AttentionSubLayer(torch.autograd.Function):
     """``y = dense(flash_alibi_attention(qkv(LayerNorm(x)))) + x`` as ONE autograd node (native path):
-    LN kernel, (AG->)GEMM+bias, tcgen05 flash attention, GEMM(->RS)+bias+residual.  The residual-stream
+    LN kernel, (AG->)GEMM+bias, wgmma flash attention, GEMM(->RS)+bias+residual.  The residual-stream
     gradient is added inside the LN backward kernel instead of by an autograd accumulation pass."""
 
     @staticmethod
@@ -281,7 +279,7 @@ class LayerNormMLP(torch.autograd.Function):
 
 
 class Linear(torch.autograd.Function):
-    """``y = x @ W^T + b`` for any leading shape: tcgen05 GEMM (bias in the epilogue), dgrad and wgrad
+    """``y = x @ W^T + b`` for any leading shape: wgmma GEMM (bias in the epilogue), dgrad and wgrad
     GEMMs in backward.  Used by the reference-compatible Column/RowParallelLinear layers."""
 
     @staticmethod
@@ -308,7 +306,7 @@ class Linear(torch.autograd.Function):
 
 
 def linear(x, weight, bias=None):
-    """Drop-in for ``F.linear`` that runs on the sm_100a GEMM when ``x`` is a CUDA bf16 tensor."""
+    """Drop-in for ``F.linear`` that runs on the sm_90a GEMM when ``x`` is a CUDA bf16 tensor."""
     from pipegoose_b200.ops import use_native
 
     if use_native(x, weight) and weight.shape[0] % 8 == 0 and weight.shape[1] % 8 == 0:

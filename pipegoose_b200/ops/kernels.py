@@ -1,6 +1,6 @@
 """Thin functional wrappers over the native kernels with PyTorch reference fallbacks.
 
-Each wrapper has one contract and two implementations: the sm_100a kernel (CUDA bf16 tensors,
+Each wrapper has one contract and two implementations: the sm_90a kernel (CUDA bf16 tensors,
 mandatory on GPU machines) and plain PyTorch math (CPU / fp32, used by the gloo unit tests and
 as the numerics oracle in the GPU tests).
 """
@@ -304,7 +304,7 @@ def ce_finalize(logits, targets, gstats, vocab_start, grad_scale, ignore_index=-
 
 
 # ----------------------------------------------------------------------------------------------
-# ALiBi causal attention (reference math; the tcgen05 kernel lives in ops/attention.py)
+# ALiBi causal attention (reference math; the wgmma kernel lives in ops/attention.py)
 # ----------------------------------------------------------------------------------------------
 def alibi_slopes(n_head: int, device=None) -> torch.Tensor:
     """Per-head ALiBi slopes exactly as transformers' ``build_alibi_tensor`` computes them."""

@@ -1,5 +1,5 @@
 """Fused expert-parallel Switch MLP: router kernel, NVLink all-to-all dispatch fused with the token
-permute, grouped tcgen05 expert GEMMs (chunk = expert, started per expert as soon as its tokens
+permute, grouped wgmma expert GEMMs (chunk = expert, started per expert as soon as its tokens
 landed), and combine fused into the last expert GEMM's epilogue (rows scaled by the gate weight and
 stored straight into the source rank's buffer).
 

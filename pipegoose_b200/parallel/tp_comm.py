@@ -2,7 +2,7 @@
 
 Library mode (``fused=False``): NCCL/gloo all-gather / reduce-scatter around plain GEMMs — the
 correctness baseline, and what CPU tests run.  Fused mode (``fused=True``): the hand-written
-sm_100a kernels in which the collective is part of the GEMM (``pipegoose_b200.ops.comm``):
+sm_90a kernels in which the collective is part of the GEMM (``pipegoose_b200.ops.comm``):
 
     ag_gemm     all-gather -> GEMM      (column-parallel forward, row-parallel dgrad)
     gemm_rs     GEMM -> reduce-scatter  (row-parallel forward, column-parallel dgrad)
@@ -44,8 +44,7 @@ class TensorParallelComm:
 
     # 1: the collectives that have no GEMM to be fused into (vocab-parallel embedding reduce-scatter / all-gather, the
     # cross-entropy statistics exchange, the partial-gradient sum) run on the NVLink peer-memory kernels as well, so a
-    # tensor-parallel step contains no NCCL kernel.  Validated on 2 x B200 (tests/test_gpu_multi.py::test_tp2_bloom* pass,
-    # the profile of the TP2 step lists no nccl kernel, 46.38 -> 46.18 ms/step; profiles/ab_2gpu_r2.log).
+    # tensor-parallel step contains no NCCL kernel.  Covered by tests/test_gpu_multi.py::test_tp2_bloom* (2 GPUs).
     PEER_COLLECTIVES = os.environ.get("PIPEGOOSE_B200_TP_PEER_COLLECTIVES", "1") == "1"
 
     def _peer_ok(self, x: torch.Tensor) -> bool:

@@ -1,4 +1,4 @@
-"""Which (tensor, pipeline, data) layout fits a B200's 180 GB, and what does each cost?  An analytic planner (the reference
+"""Which (tensor, pipeline, data) layout fits an H100's 80 GB, and what does each cost?  An analytic planner (the reference
 has ``ProfileByMemory`` for pipeline partitions only, partitioning/profile.py; choosing the layout is left to the user).
 
 ``estimate_memory`` counts, per rank, for a Bloom-family config:
@@ -15,16 +15,16 @@ has ``ProfileByMemory`` for pipeline partitions only, partitioning/profile.py; c
   lm_head, there is no fp32 copy).
 
 ``plan`` enumerates the layouts of ``n_gpus``, drops those that cannot run (heads or blocks not divisible) and ranks the
-rest: layouts that fit first, then by an estimated relative step time built from MEASURED factors of this repository
-(``profiles/``: a tensor group of 2 costs ~12 % per step on bloom-560m, data parallelism + ZeRO-1 ~7 %, a pipeline pays
-its bubble fraction) — a guide to what to measure first, not a substitute for measuring.
+rest: layouts that fit first, then by an estimated relative step time built from two overhead factors (a tensor group
+of 2 and data parallelism + ZeRO-1, measured on bloom-560m on an earlier GPU generation and not re-measured on H100; a
+pipeline pays its bubble fraction) — a guide to what to measure first, not a substitute for measuring.
 """
 from __future__ import annotations
 
 from dataclasses import dataclass
 from typing import List, Optional
 
-from pipegoose_b200.constants import B200_HBM_BYTES
+from pipegoose_b200.constants import H100_HBM_BYTES
 
 BF16, FP32 = 2, 4
 
@@ -131,12 +131,12 @@ class Layout:
                 f"bubble {self.bubble:.2f}, est. step x{self.relative_step_time:.2f}{' — ' + self.note if self.note else ''}")
 
 
-# measured on B200s with bloom-560m, 8 x 1024 tokens per GPU (profiles/validate_*_r2.log; ROADMAP §1): step time relative
-# to one GPU.  Larger tensor groups are extrapolated per doubling; treat them as an ordering, not a prediction.
+# step time relative to one GPU of a TP2 group and of data parallelism (bloom-560m, 8 x 1024 tokens per GPU, not
+# re-measured on H100).  Larger tensor groups are extrapolated per doubling; treat them as an ordering, not a prediction.
 _TP2_COST, _DP_COST = 1.12, 1.07
 
 
-def plan(config, n_gpus: int, global_batch: int, seq_len: int, hbm_bytes: int = B200_HBM_BYTES, headroom: float = 0.9,
+def plan(config, n_gpus: int, global_batch: int, seq_len: int, hbm_bytes: int = H100_HBM_BYTES, headroom: float = 0.9,
          max_tp: int = 8, n_microbatches: Optional[int] = None, schedule: str = "1f1b") -> List[Layout]:
     """Every runnable (tp, pp, dp) of ``n_gpus`` GPUs for ``global_batch`` sequences per step, best first."""
     from pipegoose_b200.nn.pipeline_parallel.scheduler import SchedulerType, get_scheduler
@@ -178,7 +178,7 @@ def main(argv=None) -> None:
 
     from pipegoose_b200.models.bloom import BloomConfig
 
-    ap = argparse.ArgumentParser(description="rank the (tp, pp, dp) layouts of a Bloom-family model on B200s")
+    ap = argparse.ArgumentParser(description="rank the (tp, pp, dp) layouts of a Bloom-family model on H100s")
     ap.add_argument("--model", default="bloom_560m", help="a preset of BloomConfig (bloom_560m, bloom_1b7, bloom_3b, bloom_7b1) "
                     "or GPT2Config (gpt2, gpt2_medium, gpt2_large, gpt2_xl)")
     ap.add_argument("--gpus", type=int, default=8)

@@ -1,4 +1,4 @@
-"""Input pipeline helpers for 3-D parallel jobs on B200s.
+"""Input pipeline helpers for 3-D parallel jobs on GPUs.
 
 The reference leaves data loading to the user's script: a ``DistributedSampler(num_replicas=dp_size,
 rank=ctx.get_local_rank(ParallelMode.DATA))`` and a blocking ``.to("cuda")`` per step (reference

@@ -7,7 +7,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on a B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on an H100 with `-m gpu`)")
     # (pytest-timeout registers this itself; declared here so that the suite also collects cleanly without the plugin)
     config.addinivalue_line("markers", "timeout(seconds): per-test time limit of the launcher-level integration tests")
 

@@ -1,4 +1,4 @@
-"""Numerics of every sm_100a kernel against a plain PyTorch fp32 reference of the same op (GPU only)."""
+"""Numerics of every sm_90a kernel against a plain PyTorch fp32 reference of the same op (GPU only)."""
 import pytest
 import torch
 

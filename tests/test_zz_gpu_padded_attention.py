@@ -1,4 +1,4 @@
-"""Head sizes without a native tile shape (bloom-3b: D=80) on the tcgen05 flash kernel: zero-padded to D=128 with the
+"""Head sizes without a native tile shape (bloom-3b: D=80) on the wgmma flash kernel: zero-padded to D=128 with the
 softmax scale of the true width (ops/attention.py::_AlibiAttentionPadded).  Collected last on purpose."""
 import pytest
 import torch

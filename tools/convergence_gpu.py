@@ -1,4 +1,4 @@
-"""Loss curves on B200s: this library next to the reference on the same learnable synthetic task (the reference's own
+"""Loss curves on GPUs: this library next to the reference on the same learnable synthetic task (the reference's own
 "benchmarks" are convergence runs: tests/convergence/run_hybrid_parallel.py, run_ep.py — wandb + imdb, neither
 available offline).
 

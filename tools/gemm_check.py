@@ -1,4 +1,4 @@
-"""GPU dev harness: correctness of the tcgen05 GEMM in every layout/epilogue + throughput vs cuBLAS.
+"""GPU dev harness: correctness of the wgmma GEMM in every layout/epilogue + throughput vs cuBLAS.
 Writes gpurun_out/gemm_check.json."""
 import json, os, sys, time, importlib.util
 import torch
@@ -14,7 +14,7 @@ results = {"correctness": [], "perf": []}
 def gelu(x):
     return x * 0.5 * (1.0 + torch.tanh(0.79788456 * x * (1 + 0.044715 * x * x)))
 
-def run_case(M, N, K, a_mn, b_mn, bn, epi, pair=0):
+def run_case(M, N, K, a_mn, b_mn, bn, epi):
     A = torch.randn(M, K, device=dev, dtype=torch.bfloat16)
     B = torch.randn(N, K, device=dev, dtype=torch.bfloat16)
     ref = A.float() @ B.float().t()
@@ -38,7 +38,7 @@ def run_case(M, N, K, a_mn, b_mn, bn, epi, pair=0):
     elif epi == "dgelu":
         aux = torch.randn(M, N, device=dev, dtype=torch.bfloat16); flags = 32
         z = aux.float().requires_grad_(True); g = torch.autograd.grad(gelu(z).sum(), z)[0]; ref = ref * g
-    _C.gemm(a_st, b_st, out, a_mn, b_mn, bias, res, aux, flags, bn, ag={"cta_pair": pair})
+    _C.gemm(a_st, b_st, out, a_mn, b_mn, bias, res, aux, flags, bn)
     torch.cuda.synchronize()
     err = (out.float() - ref).abs().max().item()
     scale = ref.abs().max().item() + 1e-6
@@ -47,8 +47,8 @@ def run_case(M, N, K, a_mn, b_mn, bn, epi, pair=0):
     if epi == "bias_gelu":
         e2 = (aux.float() - pre).abs().max().item() / (pre.abs().max().item() + 1e-6)
         ok = ok and e2 < 2e-2
-    results["correctness"].append(dict(M=M, N=N, K=K, a_mn=a_mn, b_mn=b_mn, bn=bn, epi=epi, pair=pair, rel_err=rel, ok=bool(ok)))
-    print(("OK  " if ok else "FAIL"), M, N, K, "a_mn", a_mn, "b_mn", b_mn, "bn", bn, epi, "pair", pair, "rel", f"{rel:.2e}", flush=True)
+    results["correctness"].append(dict(M=M, N=N, K=K, a_mn=a_mn, b_mn=b_mn, bn=bn, epi=epi, rel_err=rel, ok=bool(ok)))
+    print(("OK  " if ok else "FAIL"), M, N, K, "a_mn", a_mn, "b_mn", b_mn, "bn", bn, epi, "rel", f"{rel:.2e}", flush=True)
     return ok
 
 all_ok = True
@@ -71,21 +71,6 @@ for epi in ["f32acc", "f32over"]:
     all_ok &= run_case(1024, 1024, 8192, True, True, 0, epi)
     all_ok &= run_case(512, 768, 4096, True, True, 0, epi)
     all_ok &= run_case(256, 264, 2048, True, True, 0, epi)
-# CTA-pair (cta_group::2, 256-row tiles) variants: every layout, odd sizes, every epilogue
-if stage != "nopair":
-    for (a_mn, b_mn) in [(False, False), (False, True), (True, True), (True, False)]:
-        for bn in [256, 128] + ([192] if not b_mn else []):
-            all_ok &= run_case(256, bn, 64, a_mn, b_mn, bn, "none", pair=1)
-            all_ok &= run_case(512, 512, 256, a_mn, b_mn, bn, "none", pair=1)
-            all_ok &= run_case(1024, 328, 520, a_mn, b_mn, bn, "none", pair=1)
-        all_ok &= run_case(4096, 1024, 1024, a_mn, b_mn, 0, "none", pair=1)
-        if not a_mn:
-            all_ok &= run_case(1000, 264, 200, a_mn, b_mn, 0, "none", pair=1)  # ragged M: second CTA half empty
-            all_ok &= run_case(384, 256, 128, a_mn, b_mn, 0, "none", pair=1)   # odd number of 128-row blocks
-    for epi in ["bias", "bias_gelu", "bias_res", "f32acc", "f32over", "dgelu"]:
-        all_ok &= run_case(2048, 1024, 512, False, False, 0, epi, pair=1)
-        all_ok &= run_case(640, 328, 136, False, False, 128, epi, pair=1)
-    all_ok &= run_case(1024, 1024, 8192, True, True, 0, "f32acc", pair=1)
 results["all_ok"] = bool(all_ok)
 
 def bench(fn, iters=20):
@@ -101,7 +86,6 @@ def bench(fn, iters=20):
     ts.sort()
     return ts[len(ts) // 2], ts[0]
 
-PAIR = [0]
 # fused-epilogue GEMMs at the flagship (bloom-560m, 8192 tokens) shapes
 def epi_perf():
     M, h = 8192, 1024
@@ -118,27 +102,24 @@ def epi_perf():
     g1 = torch.zeros(h, h, device=dev, dtype=torch.float32)
     g4 = torch.zeros(4 * h, h, device=dev, dtype=torch.float32)
     cases = {
-        "fc1_bias_gelu_aux": (lambda: _C.gemm(x, w1, o4, False, False, b4, None, z4, 2, ag={"cta_pair": PAIR[0]}), 2.0 * M * h * 4 * h),
-        "fc1_bias_only": (lambda: _C.gemm(x, w1, o4, False, False, b4, None, None, 0, ag={"cta_pair": PAIR[0]}), 2.0 * M * h * 4 * h),
-        "fc2_bias_residual": (lambda: _C.gemm(x4, w2, o1, False, False, b1, x, None, 0, ag={"cta_pair": PAIR[0]}), 2.0 * M * h * 4 * h),
-        "dense_bias_residual": (lambda: _C.gemm(x, wd, o1, False, False, b1, x, None, 0, ag={"cta_pair": PAIR[0]}), 2.0 * M * h * h),
-        "fc2_dgrad_dgelu": (lambda: _C.gemm(x, w2, o4, False, True, None, None, z4, 32, ag={"cta_pair": PAIR[0]}), 2.0 * M * h * 4 * h),
-        "fc1_dgrad": (lambda: _C.gemm(x4, w1, o1, False, True, ag={"cta_pair": PAIR[0]}), 2.0 * M * h * 4 * h),
-        "dense_dgrad": (lambda: _C.gemm(x, wd, o1, False, True, ag={"cta_pair": PAIR[0]}), 2.0 * M * h * h),
-        "dense_wgrad_f32acc": (lambda: _C.gemm(x, x, g1, True, True, None, None, None, 16, ag={"cta_pair": PAIR[0]}), 2.0 * M * h * h),
-        "dense_wgrad_f32over": (lambda: _C.gemm(x, x, g1, True, True, None, None, None, 0, ag={"cta_pair": PAIR[0]}), 2.0 * M * h * h),
-        "fc1_wgrad_f32acc": (lambda: _C.gemm(x4, x, g4, True, True, None, None, None, 16, ag={"cta_pair": PAIR[0]}), 2.0 * M * h * 4 * h),
+        "fc1_bias_gelu_aux": (lambda: _C.gemm(x, w1, o4, False, False, b4, None, z4, 2), 2.0 * M * h * 4 * h),
+        "fc1_bias_only": (lambda: _C.gemm(x, w1, o4, False, False, b4, None, None, 0), 2.0 * M * h * 4 * h),
+        "fc2_bias_residual": (lambda: _C.gemm(x4, w2, o1, False, False, b1, x, None, 0), 2.0 * M * h * 4 * h),
+        "dense_bias_residual": (lambda: _C.gemm(x, wd, o1, False, False, b1, x, None, 0), 2.0 * M * h * h),
+        "fc2_dgrad_dgelu": (lambda: _C.gemm(x, w2, o4, False, True, None, None, z4, 32), 2.0 * M * h * 4 * h),
+        "fc1_dgrad": (lambda: _C.gemm(x4, w1, o1, False, True), 2.0 * M * h * 4 * h),
+        "dense_dgrad": (lambda: _C.gemm(x, wd, o1, False, True), 2.0 * M * h * h),
+        "dense_wgrad_f32acc": (lambda: _C.gemm(x, x, g1, True, True, None, None, None, 16), 2.0 * M * h * h),
+        "dense_wgrad_f32over": (lambda: _C.gemm(x, x, g1, True, True, None, None, None, 0), 2.0 * M * h * h),
+        "fc1_wgrad_f32acc": (lambda: _C.gemm(x4, x, g4, True, True, None, None, None, 16), 2.0 * M * h * 4 * h),
     }
     out = {}
     for name, (fn, fl) in cases.items():
         row = {}
-        for pair, tag in [(-1, "cta1"), (1, "cta2"), (0, "auto")]:
-            PAIR[0] = pair
-            med, best = bench(fn)
-            row[tag] = dict(ms=med, tflops=fl / med / 1e9)
+        med, best = bench(fn)
+        row["auto"] = dict(ms=med, tflops=fl / med / 1e9)
         out[name] = row
         print(name, "  ".join(f"{t}: {v['ms']*1e3:.1f} us {v['tflops']:.0f} TF" for t, v in row.items()), flush=True)
-    PAIR[0] = 0
     return out
 
 results["epi_perf"] = epi_perf()
@@ -162,9 +143,6 @@ for (M, N, K) in shapes:
         row[f"ours_bn{bn}_ms"] = med
         row[f"ours_bn{bn}_tflops"] = fl / med / 1e9
         row[f"ours_bn{bn}_best_tflops"] = fl / best / 1e9
-        med, best = bench(lambda: _C.gemm(A, B, out, False, False, None, None, None, 0, bn, ag={"cta_pair": 1}))
-        row[f"ours_pair_bn{bn}_tflops"] = fl / med / 1e9
-        row[f"ours_pair_bn{bn}_best_tflops"] = fl / best / 1e9
     # dgrad / wgrad layouts at auto BN
     Bt = B.t().contiguous()
     med, _ = bench(lambda: _C.gemm(A, Bt, out, False, True))

@@ -1,11 +1,12 @@
-"""Fused Switch-MoE layer (router kernel + NVLink dispatch + grouped tcgen05 GEMMs + scatter-combine epilogue) against
+"""Fused Switch-MoE layer (router kernel + NVLink dispatch + grouped wgmma GEMMs + scatter-combine epilogue) against
 the reference-style layer (replicated tokens, per-expert GEMMs, all-reduce combine) at bloom-560m shapes —
 BASELINE.json config #4.  (Written without GPU access; first run is its own validation.)
 
     torchrun --nnodes=1 --nproc-per-node T --master-addr 127.0.0.1 tools/moe_bench.py [--experts 8] [--tokens-per-rank 8192]
 
-Times are CUDA-event, max over ranks; the roofline of the fused layer is the slower of the expert FLOPs at the measured
-bf16 peak and the dispatch + combine bytes over NVLink at 770 GB/s per direction.  Writes gpurun_out/moe_bench_T{T}.json.
+Times are CUDA-event, max over ranks; the roofline of the fused layer is the slower of the expert FLOPs at the H100
+data-sheet dense bf16 peak and the dispatch + combine bytes over NVLink at its data-sheet 450 GB/s per direction.  Rank 0
+prints the result as one JSON line and, with --out PATH, also writes it to PATH.
 """
 import argparse
 import json
@@ -16,6 +17,7 @@ import torch
 import torch.distributed as dist
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from pipegoose_b200.constants import H100_BF16_DENSE_FLOPS, H100_NVLINK_BYTES_PER_S  # noqa: E402
 from pipegoose_b200.distributed import ParallelContext  # noqa: E402
 from pipegoose_b200.models.bloom import BloomConfig, BloomMLP  # noqa: E402
 from pipegoose_b200.nn.expert_parallel import SwitchNoisePolicy, Top1Router, Top2Router  # noqa: E402
@@ -45,6 +47,7 @@ def main():
     ap.add_argument("--top-k", type=int, default=1)
     ap.add_argument("--hidden", type=int, default=1024)
     ap.add_argument("--tokens-per-rank", type=int, default=8192)
+    ap.add_argument("--out", default=None, help="also write the result JSON to this path (rank 0)")
     args = ap.parse_args()
     T = int(os.environ["WORLD_SIZE"])
     ctx = ParallelContext.from_torch(tensor_parallel_size=T, pipeline_parallel_size=1, data_parallel_size=1, backend="nccl")
@@ -83,15 +86,17 @@ def main():
     # roofline of the fused layer (forward + backward): expert GEMMs 3 x (2 GEMMs x 2 n k h 4h) and four all-to-alls
     flops = 3 * 2 * 2.0 * n * k * h * 4 * h
     nvl_bytes = 4 * n * k * h * 2 * (T - 1) / T
-    roof_ms = max(flops / 1459.4e12, nvl_bytes / 770e9) * 1e3
+    roof_ms = max(flops / H100_BF16_DENSE_FLOPS, nvl_bytes / H100_NVLINK_BYTES_PER_S) * 1e3
     row = dict(T=T, experts=E, top_k=k, tokens_per_rank=n, hidden=h, fused_ms=t_fused, reference_style_ms=t_plain,
                roofline_ms=roof_ms, fused_frac_of_roofline=roof_ms / t_fused,
-               bound="link" if nvl_bytes / 770e9 > flops / 1459.4e12 else "compute",
+               bound="link" if nvl_bytes / H100_NVLINK_BYTES_PER_S > flops / H100_BF16_DENSE_FLOPS else "compute",
                note="reference-style layer processes T x the tokens per rank (replicated activations) and combines with an all-reduce")
     if rank == 0:
         print(json.dumps(row), flush=True)
-        os.makedirs("gpurun_out", exist_ok=True)
-        json.dump(row, open(f"gpurun_out/moe_bench_T{T}.json", "w"), indent=1)
+        if args.out:
+            os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+            with open(args.out, "w") as f:
+                json.dump(row, f, indent=1)
     ctx.destroy()
 
 

@@ -13,11 +13,11 @@ if which == "gemm":
     out = torch.empty(M, N, device=dev, dtype=torch.bfloat16); aux = torch.empty_like(out)
     for _ in range(6): n.gemm(a, b, out, False, False, bias, None, aux, 2)
 elif which == "gemm_pair":
-    # lm_head-like (long N) shape: the host picks CTA pairs (tcgen05 cta_group::2, 256 x 256 tiles)
+    # lm_head-like (long N) shape
     M, N, Kd = 8192, 32768, 1024
     a = torch.randn(M, Kd, device=dev, dtype=torch.bfloat16); b = torch.randn(N, Kd, device=dev, dtype=torch.bfloat16)
     out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-    for _ in range(6): n.gemm(a, b, out, ag={"cta_pair": 1})
+    for _ in range(6): n.gemm(a, b, out)
 elif which == "gemm_big":
     M = N = Kd = 8192
     a = torch.randn(M, Kd, device=dev, dtype=torch.bfloat16); b = torch.randn(N, Kd, device=dev, dtype=torch.bfloat16)

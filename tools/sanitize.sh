@@ -1,9 +1,9 @@
 #!/usr/bin/env bash
 # compute-sanitizer targets for the hand-written kernels (the reference ships no sanitizer usage, SURVEY §5.2).
-# Run on a B200 box, one GPU:   gpurun --timeout 1500 -- 'bash tools/sanitize.sh memcheck'
+# Run on one GPU:   bash tools/sanitize.sh memcheck
 #   memcheck  : out-of-bounds / misaligned global+shared accesses (TMA boxes, swizzled staging, peer stores)
-#   racecheck : shared-memory hazards between the producer / MMA / epilogue roles (mbarrier-ordered hand-offs)
-#   synccheck : invalid barrier usage (bar.sync 1,256 in the reduce-scatter epilogue, cluster barriers)
+#   racecheck : shared-memory hazards between the producer / consumer / epilogue roles (mbarrier-ordered hand-offs)
+#   synccheck : invalid barrier usage (named barriers of the GEMM epilogue)
 # The kernel tests are tiny shapes, so a run is minutes even at sanitizer speed.  Multi-GPU flag protocols
 # (st.release.sys / ld.acquire.sys) are covered functionally by tests/test_gpu_multi.py; racecheck does not model
 # cross-GPU traffic.

@@ -1,4 +1,4 @@
-"""Per-kernel SASS evidence (runs here, no GPU): counts of the mnemonics that prove the Blackwell / NVLink paths.
+"""Per-kernel SASS evidence (runs here, no GPU): counts of the mnemonics that prove the Hopper / NVLink paths.
 
     python tools/sass_summary.py > profiles/sass_summary.txt
 """
@@ -8,7 +8,7 @@ import subprocess
 import sys
 
 SO = sys.argv[1] if len(sys.argv) > 1 else "pipegoose_b200/_C.so"
-KEEP = ("UTCHMMA", "UTCQMMA", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "UTCBAR", "SYNCS", "LDGMC", "STGMC", "REDGMC",
+KEEP = ("HGMMA", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "LDGMC", "STGMC", "REDGMC",
         "REDG", "ATOMG", "MUFU", "LDG", "STG", "HMMA", "USETMAXREG", "ACQBULK", "PREEXIT", "CCTL")
 sass = subprocess.run(["cuobjdump", "-sass", SO], capture_output=True, text=True).stdout
 demangle = {}
@@ -30,17 +30,13 @@ for line in sass.splitlines():
         for k in KEEP:
             if op == k or op.startswith(k):
                 key = k
-                if k == "UTCHMMA" and ".2CTA" in mods:
-                    key = "UTCHMMA.2CTA"
-                if k == "UTMALDG" and ".2CTA" in mods:
-                    key = "UTMALDG.2CTA"
                 if k in ("STG", "LDG") and ".MC" in mods:   # multimem.st shows as a multicast-qualified store
                     key = k + ".MC"
                 counts[cur][key] += 1
                 break
-print("# SASS evidence per kernel (cuobjdump -sass pipegoose_b200/_C.so; sm_100a) — tools/sass_summary.py")
-print("# UTCHMMA = tcgen05.mma (.2CTA: cta_group::2), LDTM/STTM = tcgen05.ld/st, UTMALDG/UTMASTG = TMA tensor load/store,")
-print("# UBLKCP = cp.async.bulk, UTCBAR = tcgen05.commit, SYNCS = mbarrier ops, LDGMC = multimem.ld_reduce (NVLS),")
+print("# SASS evidence per kernel (cuobjdump -sass pipegoose_b200/_C.so; sm_90a) — tools/sass_summary.py")
+print("# HGMMA = wgmma.mma_async, UTMALDG/UTMASTG = TMA tensor load/store,")
+print("# UBLKCP = cp.async.bulk, SYNCS = mbarrier ops, LDGMC = multimem.ld_reduce (NVLS),")
 print("# (multimem.st compiles to STG.E.128.STRONG.SYS on the multicast address: the aperture, not the opcode, selects NVLS),")
 print("# REDG = red.global (peer or local), USETMAXREG = setmaxnreg, ACQBULK / PREEXIT = griddepcontrol (PDL)")
 print()

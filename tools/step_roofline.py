@@ -1,10 +1,10 @@
 """Speed-of-light table of one training step, from MEASURED inputs only (runs here, no GPU):
 
-    python tools/step_roofline.py profiles/step_breakdown_560m_1gpu_r2.json > profiles/step_roofline_560m_1gpu_r2.md
+    python tools/step_roofline.py <step breakdown .json from tools/step_profile.py> > <table>.md
 
-* kernel times: a per-kernel summary of one profiled step (``tools/step_profile.py`` on a B200, committed under
-  ``profiles/``);
-* denominators: ``MEASURED_PEAKS.json`` (driver-written: copy bandwidth and cuBLAS bf16 throughput of the same part);
+* kernel times: a per-kernel summary of one profiled step (``tools/step_profile.py --aggregate`` on the GPU);
+* denominators: ``MEASURED_PEAKS.json`` at the repository root (copy bandwidth and cuBLAS bf16 throughput measured on the
+  same part; ``bf16_tflops``, ``bf16_tflops_sustained``, ``hbm_gbs``);
 * numerators: FLOPs / bytes every kernel class MUST do for the benchmark's model and batch (formulas below, nothing
   fitted).
 
@@ -19,7 +19,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def main():
-    path = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "profiles", "step_breakdown_560m_1gpu_r2.json")
+    if len(sys.argv) < 2:
+        raise SystemExit("usage: python tools/step_roofline.py <step breakdown .json>")
+    path = sys.argv[1]
     prof = json.load(open(path))
     peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     tf = peaks["bf16_tflops_sustained"] * 1e12          # FLOP/s, back-to-back cuBLAS bf16 (what a step can sustain)
@@ -40,7 +42,7 @@ def main():
     act = M * h * 2                                                          # one [tokens, h] bf16 activation
     rows = {
         # name: (kernel-name fragments, FLOPs, bytes, note)
-        "GEMM forward (NT, 96 layer + lm_head)": (["gemm_bf16_kernel<256, 0, 0"], gemm_pass, 0, "tcgen05, cta_group::2"),
+        "GEMM forward (NT, 96 layer + lm_head)": (["gemm_bf16_kernel<256, 0, 0"], gemm_pass, 0, "wgmma"),
         "GEMM dgrad (NN)": (["gemm_bf16_kernel<256, 0, 1"], gemm_pass, 0, ""),
         "GEMM wgrad (TN, fp32 main-grad accumulate)": (["gemm_bf16_kernel<256, 1, 1"], gemm_pass, 0, ""),
         "attention forward": (["attention_fwd_kernel"], attn_fwd, L * (3 * act + act), "flash, ALiBi in-kernel"),
@@ -59,7 +61,7 @@ def main():
     total = prof["total_us"]
     used = set()
     out = []
-    out.append(f"# Step roofline: bloom-560m, {B} x {S} tokens, 1 x B200 ({os.path.basename(path)})\n")
+    out.append(f"# Step roofline: bloom-560m, {B} x {S} tokens, 1 GPU ({os.path.basename(path)})\n")
     out.append(f"Denominators (MEASURED_PEAKS.json): bf16 sustained {peaks['bf16_tflops_sustained']:.0f} TFLOP/s "
                f"(burst {peaks['bf16_tflops']:.0f}), copy bandwidth {peaks['hbm_gbs']:.0f} GB/s.  "
                f"Profiled step: {total / 1e3:.2f} ms in {prof['launches']} launches.\n")

@@ -6,6 +6,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from pipegoose_b200.distributed import ParallelContext, ParallelMode
 from pipegoose_b200.parallel.tp_comm import TensorParallelComm
 from pipegoose_b200.ops import kernels as K
+from pipegoose_b200.constants import H100_BF16_DENSE_FLOPS, H100_NVLINK_BYTES_PER_S
 
 T = int(os.environ["WORLD_SIZE"])
 ctx = ParallelContext.from_torch(tensor_parallel_size=T, pipeline_parallel_size=1, data_parallel_size=1, backend="nccl")
@@ -52,8 +53,8 @@ for name, kind, N, Kd in [("qkv", "ag", 3 * h // T, h), ("fc1", "ag", 4 * h // T
         coll_only = timeit(lambda: comm.reduce_scatter_rows(part))
         nvl_bytes = (T - 1) * (M // T) * N * 2
     flops = 2.0 * M * N * Kd
-    t_flops = flops / 1459.4e12 * 1e3   # ms at measured sustained bf16 peak
-    t_link = nvl_bytes / 770e9 * 1e3    # ms at measured 770 GB/s per direction
+    t_flops = flops / H100_BF16_DENSE_FLOPS * 1e3   # ms at the data-sheet dense bf16 peak
+    t_link = nvl_bytes / H100_NVLINK_BYTES_PER_S * 1e3    # ms at the data-sheet NVLink bandwidth per direction
     roof = max(t_flops, t_link)
     rows.append(dict(op=name, kind=kind, M=M, N=N, K=Kd, T=T, fused_ms=fused, nccl_plus_gemm_ms=lib, gemm_only_ms=gemm_only,
                      collective_only_ms=coll_only, roofline_ms=roof, fused_frac_of_roofline=roof / fused,
