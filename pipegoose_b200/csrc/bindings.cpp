@@ -55,6 +55,8 @@ void gemm(const torch::Tensor& a, const torch::Tensor& b, torch::Tensor out, boo
   d.out = out.data_ptr();
   d.ldc = (int)out.stride(0);
   TORCH_CHECK(d.ldc % 8 == 0, "out leading dimension must be a multiple of 8");
+  // both epilogues write 16-byte groups (vector stores / TMA)
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(d.out) % 16 == 0, "out must be 16B aligned");
   d.flags = (int)flags | (f32 ? 8 : 0);
   if (bias.has_value()) {
     TORCH_CHECK(bias->scalar_type() == torch::kBFloat16 && bias->numel() % N == 0 && bias->is_contiguous(), "bias must be contiguous bf16 [N] (or [groups, N])");

@@ -106,11 +106,16 @@ static int num_sms() {
   return n;
 }
 
-template <int BN, bool A_MN, bool B_MN>
-static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tal,
+// The three tensor maps of the TMA-store epilogue ([64 x 64] boxes over out / aux / the epilogue input)
+struct EpiMaps {
+  CUtensorMap out, aux, in;
+};
+
+template <int BN, bool A_MN, bool B_MN, bool TMA_EPI>
+static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tal, const EpiMaps& em,
                       const GemmArgs& args, int max_ctas, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
-  auto kern = gemm_bf16_kernel<BN, A_MN, B_MN>;
+  using Cfg = GemmCfg<BN, TMA_EPI>;
+  auto kern = gemm_bf16_kernel<BN, A_MN, B_MN, TMA_EPI>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e =
@@ -140,7 +145,7 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const CUtens
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, tal, args);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ta, tb, tal, em.out, em.aux, em.in, args);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) {
     fprintf(stderr, "pipegoose_b200: gemm launch failed: %s\n", cudaGetErrorString(e));
@@ -303,22 +308,50 @@ extern "C" int pg_gemm_bf16(const PgGemmDesc* d, cudaStream_t stream) {
     args.a_local_chunk = d->my_rank;
   }
 
-#define PG_DISPATCH_BN(AMN, BMN)                                                           \
-  switch (bn) {                                                                            \
-    case 256: return launch_cfg<256, AMN, BMN>(ta, tb, tal, args, max_ctas, stream);        \
-    case 192: return launch_cfg<192, AMN, BMN>(ta, tb, tal, args, max_ctas, stream);        \
-    case 128: return launch_cfg<128, AMN, BMN>(ta, tb, tal, args, max_ctas, stream);        \
-    case 64: return launch_cfg<64, AMN, BMN>(ta, tb, tal, args, max_ctas, stream);          \
-    default: fprintf(stderr, "pipegoose_b200: bad block_n %d\n", bn); return -1;           \
+  // The TMA-store epilogue serves every call with a bf16 output, one chunk (no fused collective, no MoE scatter)
+  // and 16-byte-aligned matrices (TMA's requirement).  The GELU pre-activation output cannot share the slots with
+  // an epilogue input, so that combination also stays on the general epilogue.
+  auto aligned = [](const void* p, int ld) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0 && (ld % 8) == 0; };
+  const void* epi_in = (args.flags & EPI_DGELU) ? args.aux : (args.flags & EPI_RESIDUAL) ? args.residual : nullptr;
+  const int in_ld = (args.flags & EPI_DGELU) ? args.ldc : args.ldr;
+  const bool gelu_aux = (args.flags & EPI_GELU) && args.aux != nullptr;
+  const bool tma_epi = !(args.flags & (EPI_OUT_F32 | EPI_SCATTER)) && args.num_chunks == 1 && args.n_comm == 0 &&
+                       args.grad_rs.world <= 1 && args.k_splits == 1 && aligned(args.out, args.ldc) &&
+                       (!gelu_aux || (aligned(args.aux, args.ldc) && epi_in == nullptr)) &&
+                       (epi_in == nullptr || aligned(epi_in, in_ld)) &&
+                       (!(args.flags & EPI_BIAS) || aligned(args.bias, 8));
+  EpiMaps em;
+  memset(&em, 0, sizeof(em));
+  if (tma_epi) {
+    if (cached_tmap(&em.out, args.out, args.M, args.N, args.ldc, 64) != 0) return -1;
+    em.aux = em.in = em.out;
+    if (gelu_aux && cached_tmap(&em.aux, args.aux, args.M, args.N, args.ldc, 64) != 0) return -1;
+    if (epi_in != nullptr && cached_tmap(&em.in, epi_in, args.M, args.N, in_ld, 64) != 0) return -1;
+  }
+
+#define PG_DISPATCH_BN(AMN, BMN, EPI)                                                                    \
+  switch (bn) {                                                                                          \
+    case 256: return launch_cfg<256, AMN, BMN, EPI>(ta, tb, tal, em, args, max_ctas, stream);             \
+    case 192: return launch_cfg<192, AMN, BMN, EPI>(ta, tb, tal, em, args, max_ctas, stream);             \
+    case 128: return launch_cfg<128, AMN, BMN, EPI>(ta, tb, tal, em, args, max_ctas, stream);             \
+    case 64: return launch_cfg<64, AMN, BMN, EPI>(ta, tb, tal, em, args, max_ctas, stream);               \
+    default: fprintf(stderr, "pipegoose_b200: bad block_n %d\n", bn); return -1;                         \
+  }
+#define PG_DISPATCH_EPI(AMN, BMN) \
+  if (tma_epi) {                  \
+    PG_DISPATCH_BN(AMN, BMN, true) \
+  } else {                        \
+    PG_DISPATCH_BN(AMN, BMN, false) \
   }
   if (!d->a_mn && !d->b_mn) {
-    PG_DISPATCH_BN(false, false)
+    PG_DISPATCH_EPI(false, false)
   } else if (!d->a_mn && d->b_mn) {
-    PG_DISPATCH_BN(false, true)
+    PG_DISPATCH_EPI(false, true)
   } else if (d->a_mn && d->b_mn) {
-    PG_DISPATCH_BN(true, true)
+    PG_DISPATCH_EPI(true, true)
   } else {
-    PG_DISPATCH_BN(true, false)
+    PG_DISPATCH_EPI(true, false)
   }
+#undef PG_DISPATCH_EPI
 #undef PG_DISPATCH_BN
 }

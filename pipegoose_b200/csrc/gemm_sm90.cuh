@@ -1,7 +1,8 @@
 // Persistent, warp-specialised bf16 GEMM for sm_90a:
 //   TMA (cp.async.bulk.tensor) -> 128B-swizzled smem ring -> wgmma.mma_async issued by two
 //   consumer warpgroups (64 rows of the 128-row tile each, fp32 accumulators in registers) ->
-//   epilogue by the same warpgroups, accumulators handed over through shared memory.
+//   epilogue by the same warpgroups: for bf16 outputs in the accumulator-fragment layout with TMA stores
+//   (epilogue_tma), otherwise accumulators handed over through shared memory (the general epilogue).
 //
 // One kernel serves the three operand layouts a transformer training step needs
 //   NT : Y  = X  · Wᵀ   (A K-major,  B K-major)    forward
@@ -97,17 +98,26 @@ struct GemmArgs {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int WG_K = 16;           // K of one wgmma instruction
-constexpr int kGemmThreads = 384;  // warpgroup 0: warp 0 TMA (warps 1-3 idle); warpgroups 1, 2: wgmma + epilogue
+constexpr int kGemmThreads = 384;  // warpgroup 0: warp 0 TMA, warp 1 epilogue-operand TMA; warpgroups 1, 2: wgmma + epilogue
 constexpr int kAccLd = 68;         // fp32 accumulator hand-over rows: 64 columns + 4 of padding (bank spread)
 
-template <int BN>
+// Shared-memory budget.  TMA_EPI = false (general epilogue): the per-warp staging buffers and the fp32 accumulator
+// hand-over.  TMA_EPI = true (TMA-store epilogue): the whole 128 x BN bf16 output tile as [64 x 64] 128B-swizzled
+// slots (slot 2-D index: warpgroup, 64-column group) plus the tile's bias slice; the slots first receive the
+// tile's residual / GELU' input and are then overwritten in place by the output.  The stage count is what is left:
+// 3 at BN = 256 and 4 at BN = 192 (as for the general epilogue), 6 at BN = 128, 8 at BN = 64.
+template <int BN, bool TMA_EPI = false>
 struct GemmCfg {
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kEpiStageBytes = 8 * 32 * 64;                // 8 epilogue warps x [32 rows x 64 B]
-  static constexpr int kAccStageBytes = 2 * 64 * kAccLd * 4;        // per consumer warpgroup: [64 rows x 64 cols] fp32
-  static constexpr int kFixedBytes = kEpiStageBytes + kAccStageBytes + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int kEpiStageBytes = TMA_EPI ? 0 : 8 * 32 * 64;  // 8 epilogue warps x [32 rows x 64 B]
+  static constexpr int kAccStageBytes = TMA_EPI ? 0 : 2 * 64 * kAccLd * 4;  // per consumer warpgroup: [64 x 64] fp32
+  static constexpr int kSlotBytes = 64 * 64 * 2;
+  static constexpr int kSlots = TMA_EPI ? 2 * (BN / 64) : 0;
+  static constexpr int kBiasBytes = TMA_EPI ? BN * 2 : 0;
+  static constexpr int kFixedBytes =
+      kEpiStageBytes + kAccStageBytes + kSlots * kSlotBytes + kBiasBytes + 1024 /*align*/ + 256 /*barriers*/;
   static constexpr int kMaxStages = (227 * 1024 - kFixedBytes) / kStageBytes;  // 227 KB: sm_90 opt-in maximum
   static constexpr int kStages = kMaxStages > 8 ? 8 : kMaxStages;
   static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
@@ -154,18 +164,165 @@ PG_DEVICE TileCoord map_tile(int t, int m_blks_per_chunk, int n_blks, int num_ch
   return c;
 }
 
+// The bf16 matrix the epilogue reads element-wise (GELU' pre-activation or residual; the same choice in both
+// epilogues), null: none.
+PG_DEVICE const void* epi_input(const GemmArgs& a) {
+  return (a.flags & EPI_DGELU) ? a.aux : (a.flags & EPI_RESIDUAL) ? static_cast<const void*>(a.residual) : nullptr;
+}
+
+// TMA-store epilogue of one tile for consumer warpgroup wg (tile rows [64 wg, 64 wg + 64)), bf16 output, one chunk.
+// Bias, cross-entropy partials, GELU (+ pre-activation), GELU' and residual are applied in fp32 on the accumulator
+// fragments with the general epilogue's arithmetic, in its order, so the bf16 results are the same bits.  The
+// bias slice and the residual / GELU' input were loaded into shared memory by the producer warpgroup under the main
+// loop (epi_full).  The bf16 results are written in place into the warpgroup's 128B-swizzled [64 x 64] slots and
+// leave with TMA stores (clipped at the M / N edges) that nobody waits for here: the storing thread waits for
+// them to have READ the slots during the next tile's first k-block, or at kernel exit.
+//
+// Fragment element acc[4 j + 2 hh + e] is row 16 wl + lane / 4 + 8 hh, column 8 j + 2 (lane % 4) + e of the
+// warpgroup's 64 x BN block (wgmma.cuh); the pair (e = 0, 1) is one 4-byte word of slot j / 8, whose 16-byte chunk
+// j % 8 of row r sits at chunk (j % 8) ^ (r % 8) (r % 8 = lane / 4): the 32 lanes of a warp hit 32 different banks.
+template <int BN>
+PG_DEVICE void epilogue_tma(float (&acc)[BN / 2], const GemmArgs& args, const CUtensorMap* tma_out,
+                            const CUtensorMap* tma_aux, uint8_t* wslots, const uint8_t* bias_s, uint64_t* epi_full,
+                            uint32_t epi_parity, bool has_in, int m_blk, int n_blk, int n_blks, int wg, int tid_wg) {
+  constexpr int kSlotBytes = 64 * 64 * 2;
+  const int lane = tid_wg & 31;
+  const int wl = tid_wg >> 5;
+  const int quad = lane & 3;
+  const int m0 = m_blk * BM + 64 * wg;
+  const int n0 = n_blk * BN;
+  uint8_t* my_row = wslots + (16 * wl + (lane >> 2)) * 128 + quad * 4;
+  auto word = [&](int j, int hh) -> uint32_t* {
+    return reinterpret_cast<uint32_t*>(my_row + (j >> 3) * kSlotBytes + hh * (8 * 128) + (((j & 7) ^ (lane >> 2)) << 4));
+  };
+  auto store_tile = [&](const CUtensorMap* map) {
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) *word(j, hh) = pack_bf16x2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]);
+    fence_proxy_async_smem();
+    named_bar_sync(2 + wg, 128);
+    if (tid_wg == 0) {
+#pragma unroll
+      for (int s = 0; s < BN / 64; ++s) tma_store_2d(map, wslots + s * kSlotBytes, n0 + 64 * s, m0);
+      tma_store_commit();
+    }
+  };
+
+  if (has_in) {
+    mbar_wait(epi_full, epi_parity);
+  } else {
+    named_bar_sync(2 + wg, 128);  // the storing thread saw the previous tile's stores read the slots
+  }
+  if (args.flags & EPI_BIAS) {
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(bias_s + (8 * j + 2 * quad) * 2));
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        acc[4 * j + 2 * hh] += b.x;
+        acc[4 * j + 2 * hh + 1] += b.y;
+      }
+    }
+  }
+  if (args.ce_part != nullptr) {
+    // statistics of the values as they are STORED (rounded to bf16); per row and tile half [BN/2 h, BN/2 (h + 1)):
+    // each thread of a quad holds a quarter of the row's columns, the quad merges them with shuffles
+    const int lim = min(args.N, args.ce_valid) - n0;  // columns [0, lim) of the tile enter the statistics
+    float mx[2][2], sm[2][2];                         // [hh][half]
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        mx[hh][hf] = -INFINITY;
+        sm[hh][hf] = 0.f;
+      }
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& v = acc[4 * j + 2 * hh + e];
+          v = __bfloat162float(__float2bfloat16_rn(v));
+          if (8 * j + 2 * quad + e < lim) mx[hh][j >= BN / 16] = fmaxf(mx[hh][j >= BN / 16], v);
+        }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        mx[hh][hf] = fmaxf(mx[hh][hf], __shfl_xor_sync(0xffffffffu, mx[hh][hf], 1));
+        mx[hh][hf] = fmaxf(mx[hh][hf], __shfl_xor_sync(0xffffffffu, mx[hh][hf], 2));
+      }
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (8 * j + 2 * quad + e < lim)
+            sm[hh][j >= BN / 16] += exp2f((acc[4 * j + 2 * hh + e] - mx[hh][j >= BN / 16]) * 1.4426950408889634f);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        sm[hh][hf] += __shfl_xor_sync(0xffffffffu, sm[hh][hf], 1);
+        sm[hh][hf] += __shfl_xor_sync(0xffffffffu, sm[hh][hf], 2);
+      }
+    // lane 4 i + hh writes row 16 wl + i + 8 hh: both halves of the tile, slots 2 n_blk and 2 n_blk + 1
+    const int row = m0 + 16 * wl + (lane >> 2) + 8 * quad;
+    if (quad < 2 && row < args.M) {
+      const float4 v = quad == 0 ? make_float4(mx[0][0], sm[0][0], mx[0][1], sm[0][1])
+                                 : make_float4(mx[1][0], sm[1][0], mx[1][1], sm[1][1]);
+      *reinterpret_cast<float4*>(args.ce_part + (static_cast<size_t>(row) * n_blks + n_blk) * 4) = v;
+    }
+  }
+  if (args.flags & EPI_GELU) {
+    if (args.aux != nullptr) store_tile(tma_aux);  // the pre-activation
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = gelu_tanh(acc[i]);
+    if (args.aux != nullptr) {
+      if (tid_wg == 0) tma_store_wait_read<0>();
+      named_bar_sync(2 + wg, 128);
+    }
+  }
+  if (epi_input(args) != nullptr) {
+    const bool dgelu = (args.flags & EPI_DGELU) != 0;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const float2 z = unpack_bf16x2(*word(j, hh));
+        if (dgelu) {
+          acc[4 * j + 2 * hh] *= gelu_tanh_grad(z.x);
+          acc[4 * j + 2 * hh + 1] *= gelu_tanh_grad(z.y);
+        } else {
+          acc[4 * j + 2 * hh] += z.x;
+          acc[4 * j + 2 * hh + 1] += z.y;
+        }
+      }
+  }
+  store_tile(tma_out);
+}
+
 // Register budget: the block owns the SM's register file (384 threads x 168 at launch); the producer warpgroup gives
 // registers back (40) and the two consumer warpgroups take them (232): 128*40 + 256*232 <= 64 K.  A consumer thread
 // holds BN/2 fp32 accumulators (128 at BN = 256) plus the epilogue's working set.
 constexpr int kGemmLightRegs = 40;
 constexpr int kGemmConsumerRegs = 232;
 
-template <int BN, bool A_MN, bool B_MN>
+// TMA_EPI selects the epilogue (the host picks the TMA-store one for every bf16-output, single-chunk call with
+// 16-byte-aligned matrices, see gemm_sm90.cu); the producer and the main loop are the same for both.
+// tma_out / tma_aux / tma_in ([64 x 64] boxes, 128B swizzle over out, aux and epi_input()) are read only by it.
+template <int BN, bool A_MN, bool B_MN, bool TMA_EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a,
                      const __grid_constant__ CUtensorMap tma_b,
-                     const __grid_constant__ CUtensorMap tma_a_local, const GemmArgs args) {
-  using Cfg = GemmCfg<BN>;
+                     const __grid_constant__ CUtensorMap tma_a_local,
+                     const __grid_constant__ CUtensorMap tma_out,
+                     const __grid_constant__ CUtensorMap tma_aux,
+                     const __grid_constant__ CUtensorMap tma_in, const GemmArgs args) {
+  using Cfg = GemmCfg<BN, TMA_EPI>;
   constexpr int STAGES = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -174,9 +331,16 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
   uint8_t* smem_b = smem + STAGES * Cfg::kABytes;
   uint8_t* smem_epi = smem + STAGES * Cfg::kStageBytes;
   float* smem_acc = reinterpret_cast<float*>(smem_epi + Cfg::kEpiStageBytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_epi + Cfg::kEpiStageBytes + Cfg::kAccStageBytes);
+  uint8_t* smem_slots = smem_epi;  // TMA_EPI: kSlots x [64 x 64] bf16, then the bias slice
+  uint8_t* smem_bias = smem_slots + Cfg::kSlots * Cfg::kSlotBytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_epi + Cfg::kEpiStageBytes + Cfg::kAccStageBytes +
+                                               Cfg::kSlots * Cfg::kSlotBytes + Cfg::kBiasBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
+  uint64_t* epi_full = bars + 2 * STAGES;       // TMA_EPI: the tile's bias / epilogue input landed in smem
+  uint64_t* epi_empty = bars + 2 * STAGES + 1;  // TMA_EPI: both warpgroups' previous stores have read the slots
+  // TMA_EPI: the producer warpgroup prefetches epilogue operands (uniform over the grid)
+  const bool has_in = TMA_EPI && ((args.flags & EPI_BIAS) || epi_input(args) != nullptr);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -262,11 +426,20 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
+    if constexpr (TMA_EPI) {
+      tma_prefetch_desc(&tma_out);
+      tma_prefetch_desc(&tma_aux);
+      tma_prefetch_desc(&tma_in);
+    }
   }
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 2);  // one arrival per consumer warpgroup
+    }
+    if constexpr (TMA_EPI) {
+      mbar_init(epi_full, 1);
+      mbar_init(epi_empty, 2);
     }
     fence_mbar_init();
   }
@@ -329,13 +502,37 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         }
       }
     }
+  } else if (TMA_EPI && warp == 1 && has_in) {
+    // ============================ epilogue operand prefetch (TMA_EPI) ============================
+    // The tile's bias slice and residual / GELU' sub-tiles go into the slots as soon as both warpgroups released them
+    // (early in the tile's main loop), so the epilogue never waits on global memory.
+    const void* in = epi_input(args);
+    uint32_t parity = 0;
+    for (int t = unit0; t < num_work; t += unit_stride) {
+      const TileCoord tc = map_tile(t % num_tiles, m_blks_per_chunk, n_blks, args.num_chunks, args.first_chunk);
+      const int n0 = tc.n_blk * BN;
+      if (lane == 0) {
+        mbar_wait(epi_empty, parity ^ 1);
+        const uint32_t bias_bytes = (args.flags & EPI_BIAS) ? min(BN, args.N - n0) * 2 : 0;
+        mbar_arrive_expect_tx(epi_full, bias_bytes + (in != nullptr ? Cfg::kSlots * Cfg::kSlotBytes : 0));
+        if (bias_bytes > 0) bulk_load_1d(smem_bias, args.bias + n0, bias_bytes, epi_full);
+        if (in != nullptr) {
+#pragma unroll
+          for (int s = 0; s < Cfg::kSlots; ++s)
+            tma_load_2d(smem_slots + s * Cfg::kSlotBytes, &tma_in, epi_full, n0 + 64 * (s % (BN / 64)),
+                        tc.m_blk * BM + 64 * (s / (BN / 64)));
+        }
+      }
+      __syncwarp();
+      parity ^= 1;
+    }
   }
   } else {
     setmaxnreg_inc<kGemmConsumerRegs>();
     // ============================ consumers: wgmma main loop + epilogue ============================
     // Warpgroup wg (0, 1) computes rows [64 wg, 64 wg + 64) of the tile with m64 x BN x k16 wgmma, keeping one group
     // of four in flight: the stage of k-block kb is released once the group of kb + 1 is issued and kb's retired.
-    // Epilogue: 8 warps; warp e = 4 wg + w (w = warp in its warpgroup) owns tile rows [32q, 32q+32) with
+    // General epilogue: 8 warps; warp e = 4 wg + w (w = warp in its warpgroup) owns tile rows [32q, 32q+32) with
     // q = 2 wg + (w & 1) (one row per thread) and every second 32-column chunk (c = h, h+2, ..., h = w >> 1).  The
     // accumulators reach the row-per-thread layout through shared memory, 64 columns (two chunks) per round.  Every
     // global access is coalesced through a per-warp [32 rows x 64 B] staging buffer (16-byte chunks XOR-swizzled by
@@ -371,6 +568,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
     const int co_r = lane >> 2;                       // coalesced pattern: row inside a group of 8
     const int co_ch = lane & 3;                       // 16-byte chunk of the 64-byte segment
     bool rs_ready = false;                            // peers' partial tiles of the local chunk have landed
+    uint32_t epi_parity = 0;                          // TMA_EPI: phase of epi_full for this tile
     for (int t = unit0; t < num_work; t += unit_stride) {
       const TileCoord tc = map_tile(t % num_tiles, m_blks_per_chunk, n_blks, args.num_chunks, args.first_chunk);
       {
@@ -393,6 +591,13 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
             Wgmma<BN, A_MN, B_MN>::mma(acc, da, db, (kb > kb_begin || k > 0) ? 1u : 0u);
           }
           wgmma_commit();
+          if constexpr (TMA_EPI) {
+            // the previous tile's stores have long read the slots: hand them to the operand prefetch / next epilogue
+            if (kb == kb_begin && t != unit0 && tid_wg == 0) {
+              tma_store_wait_read<0>();
+              if (has_in) mbar_arrive(epi_empty);
+            }
+          }
           wgmma_wait<1>();
           if (prev_stage >= 0 && tid_wg == 0) mbar_arrive(&empty_bar[prev_stage]);
           prev_stage = stage;
@@ -404,6 +609,12 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
         if (prev_stage >= 0 && tid_wg == 0) mbar_arrive(&empty_bar[prev_stage]);
+      }
+      if constexpr (TMA_EPI) {
+        epilogue_tma<BN>(acc, args, &tma_out, &tma_aux, smem_slots + wg * (BN / 64) * Cfg::kSlotBytes, smem_bias,
+                         epi_full, epi_parity, has_in, tc.m_blk, tc.n_blk, n_blks, wg, tid_wg);
+        epi_parity ^= 1;
+        continue;
       }
       const int row = tc.m_blk * BM + q * 32 + lane;
       const int n0 = tc.n_blk * BN;
@@ -695,6 +906,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         }
       }
     }
+    // TMA_EPI: the last stores complete before the CTA (and its shared memory) goes away
+    if (TMA_EPI && tid_wg == 0) tma_store_wait<0>();
   }
 }
 

@@ -1,10 +1,23 @@
 """GPU dev harness: correctness of the wgmma GEMM in every layout/epilogue + throughput vs cuBLAS.
-Writes gpurun_out/gemm_check.json."""
+Writes the results as JSON to --out (default: gemm_check.json in the current directory).
+
+    python tools/gemm_check.py [all|epi] [--so path/to/_C.so] [--out results.json]
+
+--so times another build of the extension (e.g. an older commit's) with the same harness."""
 import json, os, sys, time, importlib.util
+import numpy as np
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-spec = importlib.util.spec_from_file_location("_C", os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "pipegoose_b200", "_C.so"))
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+argv = sys.argv[1:]
+def _opt(name, default):
+    if name in argv:
+        i = argv.index(name); v = argv[i + 1]; del argv[i:i + 2]; return v
+    return default
+SO = _opt("--so", os.path.join(ROOT, "pipegoose_b200", "_C.so"))
+OUT = _opt("--out", "gemm_check.json")
+spec = importlib.util.spec_from_file_location("_C", SO)
 _C = importlib.util.module_from_spec(spec); spec.loader.exec_module(_C)
 
 dev = "cuda"
@@ -52,7 +65,7 @@ def run_case(M, N, K, a_mn, b_mn, bn, epi):
     return ok
 
 all_ok = True
-stage = sys.argv[1] if len(sys.argv) > 1 else "all"
+stage = argv[0] if argv else "all"
 # smallest first: one tile, one k-block
 for (a_mn, b_mn) in [(False, False), (False, True), (True, True), (True, False)]:
     for bn in [128, 256, 64, 192]:
@@ -101,6 +114,14 @@ def epi_perf():
     z4 = torch.randn(M, 4 * h, device=dev, dtype=torch.bfloat16)
     g1 = torch.zeros(h, h, device=dev, dtype=torch.float32)
     g4 = torch.zeros(4 * h, h, device=dev, dtype=torch.float32)
+    w3 = torch.randn(3 * h, h, device=dev, dtype=torch.bfloat16)
+    b3 = torch.randn(3 * h, device=dev, dtype=torch.bfloat16)
+    o3 = torch.empty(M, 3 * h, device=dev, dtype=torch.bfloat16)
+    V = 250880  # bloom vocabulary: lm_head logits with the cross-entropy partials in the epilogue
+    wv = torch.randn(V, h, device=dev, dtype=torch.bfloat16) * 0.05
+    ov = torch.empty(M, V, device=dev, dtype=torch.bfloat16)
+    ce_part = torch.empty(M, 2 * ((V + 255) // 256), 2, device=dev, dtype=torch.float32)
+    ce_ag = {"ce_part": ce_part.data_ptr(), "ce_valid": V}
     cases = {
         "fc1_bias_gelu_aux": (lambda: _C.gemm(x, w1, o4, False, False, b4, None, z4, 2), 2.0 * M * h * 4 * h),
         "fc1_bias_only": (lambda: _C.gemm(x, w1, o4, False, False, b4, None, None, 0), 2.0 * M * h * 4 * h),
@@ -109,6 +130,8 @@ def epi_perf():
         "fc2_dgrad_dgelu": (lambda: _C.gemm(x, w2, o4, False, True, None, None, z4, 32), 2.0 * M * h * 4 * h),
         "fc1_dgrad": (lambda: _C.gemm(x4, w1, o1, False, True), 2.0 * M * h * 4 * h),
         "dense_dgrad": (lambda: _C.gemm(x, wd, o1, False, True), 2.0 * M * h * h),
+        "qkv_bias": (lambda: _C.gemm(x, w3, o3, False, False, b3, None, None, 0), 2.0 * M * h * 3 * h),
+        "lm_head_ce": (lambda: _C.gemm(x, wv, ov, False, False, None, None, None, 0, ag=ce_ag), 2.0 * M * h * V),
         "dense_wgrad_f32acc": (lambda: _C.gemm(x, x, g1, True, True, None, None, None, 16), 2.0 * M * h * h),
         "dense_wgrad_f32over": (lambda: _C.gemm(x, x, g1, True, True, None, None, None, 0), 2.0 * M * h * h),
         "fc1_wgrad_f32acc": (lambda: _C.gemm(x4, x, g4, True, True, None, None, None, 16), 2.0 * M * h * 4 * h),
@@ -120,12 +143,33 @@ def epi_perf():
         row["auto"] = dict(ms=med, tflops=fl / med / 1e9)
         out[name] = row
         print(name, "  ".join(f"{t}: {v['ms']*1e3:.1f} us {v['tflops']:.0f} TF" for t, v in row.items()), flush=True)
+    del wv, ov, ce_part
     return out
 
+# Plain NT GEMM at M = 8192, N = 4096, BN = 256 over K: time per tile round = fixed + per_kb * (K / 64).  The fit
+# separates the steady-state cost of a 64-deep k-block from the per-tile cost outside the main loop (prologue,
+# epilogue, pipeline fill).
+def k_sweep():
+    M, N, bn = 8192, 4096, 256
+    rounds = -(-((M // 128) * (N // bn)) // torch.cuda.get_device_properties(0).multi_processor_count)
+    rows = []
+    for K in (512, 1024, 2048, 4096):
+        A = torch.randn(M, K, device=dev, dtype=torch.bfloat16)
+        B = torch.randn(N, K, device=dev, dtype=torch.bfloat16)
+        out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
+        med, _ = bench(lambda: _C.gemm(A, B, out, False, False, None, None, None, 0, bn))
+        rows.append(dict(K=K, ms=med, us_per_round=med * 1e3 / rounds))
+    kb = np.array([r["K"] / 64 for r in rows]); t = np.array([r["us_per_round"] for r in rows])
+    per_kb, fixed = np.polyfit(kb, t, 1)
+    res = dict(M=M, N=N, bn=bn, rounds=rounds, rows=rows, per_kblock_us=float(per_kb), fixed_per_tile_us=float(fixed))
+    print("k_sweep", json.dumps(res), flush=True)
+    return res
+
 results["epi_perf"] = epi_perf()
+results["k_sweep"] = k_sweep()
 if stage == "epi":
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump(results, open("gpurun_out/gemm_check.json", "w"), indent=1)
+    os.makedirs(os.path.dirname(os.path.abspath(OUT)), exist_ok=True)
+    json.dump(results, open(OUT, "w"), indent=1)
     print("ALL_OK", all_ok)
     sys.exit(0)
 
@@ -154,6 +198,6 @@ for (M, N, K) in shapes:
     print(json.dumps(row), flush=True)
     del A, B, out, Bt, At
 
-os.makedirs("gpurun_out", exist_ok=True)
-json.dump(results, open("gpurun_out/gemm_check.json", "w"), indent=1)
+os.makedirs(os.path.dirname(os.path.abspath(OUT)), exist_ok=True)
+json.dump(results, open(OUT, "w"), indent=1)
 print("ALL_OK", all_ok)
