@@ -15,6 +15,12 @@
 // A operands (dV, dK accumulate in registers across the loop), and the warpgroup's share of
 // dQ = dS K (its 64 keys) from dS^T staged in shared memory, reduced into an fp32 buffer with
 // red.global.add.
+//
+// Packed sequences (SEG = true): seg_start[b*S + s] is the row-relative position where the document holding token s
+// begins (non-decreasing along a row), and query q sees key k iff seg_start[q] <= k <= q.  The forward starts its key
+// loop at the block holding the CTA's first query's document start; the backward ends its query loop at the end of the
+// document holding the key block's last key.  Key / query blocks outside those ranges hold no visible pair and are
+// never loaded.  SEG = false compiles to the kernels without the lower bound.
 #include "launch.h"
 #include "pdl_launch.cuh"
 #include "ptx.cuh"
@@ -70,9 +76,10 @@ struct AttFwdArgs {
   const float* slopes;
   int B, S, H, ld_out;
   float scale_log2;  // log2(e) / sqrt(D)
+  const int* seg_start;  // [B*S] document start of every token (SEG only)
 };
 
-template <int D>
+template <int D, bool SEG>
 __global__ void __launch_bounds__(kAttThreads, 1)
     attention_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const AttFwdArgs args) {
   using Cfg = AttFwdCfg<D>;
@@ -107,6 +114,10 @@ __global__ void __launch_bounds__(kAttThreads, 1)
   }
   __syncthreads();
   pdl_wait();  // prologue above overlapped the predecessor; Q/K/V are read below
+  // first key block with a visible pair: seg_start is non-decreasing, so the first query's document start is the CTA's
+  // lowest.  Producer and consumers run the same j0 .. num_kb - 1.
+  int j0 = 0;
+  if constexpr (SEG) j0 = args.seg_start[row0] / ATT_BN;
 
   if (warp < 4) {
     setmaxnreg_dec<kAttRegsLight>();
@@ -119,7 +130,7 @@ __global__ void __launch_bounds__(kAttThreads, 1)
       }
       int stage = 0;
       uint32_t phase = 0;
-      for (int j = 0; j < num_kb; ++j) {
+      for (int j = j0; j < num_kb; ++j) {
         mbar_wait(&kv_empty[stage], phase ^ 1);
         if (lane == 0) {
           const int krow = batch * args.S + j * ATT_BN;
@@ -148,6 +159,11 @@ __global__ void __launch_bounds__(kAttThreads, 1)
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) qpos[hh] = qb * ATT_BM + 64 * wg + 16 * wl + (lane >> 2) + 8 * hh;
   const float slope2 = args.slopes[head] * kLog2e;
+  int seg[2] = {0, 0};  // document start of each row (padded rows of the last block read the last token's)
+  if constexpr (SEG) {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) seg[hh] = args.seg_start[batch * args.S + min(qpos[hh], args.S - 1)];
+  }
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   float s[ATT_BN / 2];
   float o[D / 2];
@@ -157,7 +173,7 @@ __global__ void __launch_bounds__(kAttThreads, 1)
   mbar_wait(q_full, 0);
   int stage = 0;
   uint32_t phase = 0;
-  for (int j = 0; j < num_kb; ++j) {
+  for (int j = j0; j < num_kb; ++j) {
     mbar_wait(&kv_full[stage], phase);
     const uint32_t aK = smem_u32(sK + stage * Cfg::kTileBytes), aV = smem_u32(sV + stage * Cfg::kTileBytes);
     // S = Q K^T
@@ -178,6 +194,7 @@ __global__ void __launch_bounds__(kAttThreads, 1)
     for (int hh = 0; hh < 2; ++hh) {
       const float bias0 = slope2 * static_cast<float>(j * ATT_BN - qpos[hh]);
       const int lim = qpos[hh] - j * ATT_BN;  // column c is visible iff c <= lim
+      const int lo = seg[hh] - j * ATT_BN;    // ... and (SEG) c >= lo
       float mx = -INFINITY;
 #pragma unroll
       for (int jn = 0; jn < ATT_BN / 8; ++jn) {
@@ -186,6 +203,7 @@ __global__ void __launch_bounds__(kAttThreads, 1)
           const int col = 8 * jn + 2 * t4 + e;
           float x = fmaf(s[4 * jn + 2 * hh + e], args.scale_log2, fmaf(slope2, static_cast<float>(col), bias0));
           if (diag && col > lim) x = -INFINITY;
+          if (SEG && col < lo) x = -INFINITY;
           s[4 * jn + 2 * hh + e] = x;
           mx = fmaxf(mx, x);
         }
@@ -193,13 +211,16 @@ __global__ void __launch_bounds__(kAttThreads, 1)
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
       const float m_new = fmaxf(m_run[hh], mx);
-      const float alpha = fast_exp2(m_run[hh] - m_new);  // m_run = -inf on the first block -> 0
+      // SEG: a row whose document starts after this block has seen nothing yet (m_new = -inf); subtracting 0 keeps
+      // alpha and p at exp2(-inf) = 0 instead of exp2(-inf - -inf) = NaN
+      const float m_sub = (SEG && m_new == -INFINITY) ? 0.f : m_new;
+      const float alpha = fast_exp2(m_run[hh] - m_sub);  // m_run = -inf on the first block -> 0
       float rs = 0.f;
 #pragma unroll
       for (int jn = 0; jn < ATT_BN / 8; ++jn) {
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-          const float p = fast_exp2(s[4 * jn + 2 * hh + e] - m_new);
+          const float p = fast_exp2(s[4 * jn + 2 * hh + e] - m_sub);
           s[4 * jn + 2 * hh + e] = p;
           rs += p;
         }
@@ -305,9 +326,10 @@ struct AttBwdArgs {
   __nv_bfloat16* dqkv;      // [B*S, H*3*D]
   int B, S, H;
   float scale, scale_log2;
+  const int* seg_start;     // [B*S] document start of every token (SEG only)
 };
 
-template <int D>
+template <int D, bool SEG>
 __global__ void __launch_bounds__(kAttThreads, 1)
     attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant__ CUtensorMap tm_q,
                          const __grid_constant__ CUtensorMap tm_do, const AttBwdArgs args) {
@@ -331,7 +353,7 @@ __global__ void __launch_bounds__(kAttThreads, 1)
   const int jb = blockIdx.x;  // key block
   const int head = blockIdx.y, batch = blockIdx.z;
   const int qb0 = jb * (ATT_BN / ATT_BWD_BM);  // first query block that sees these keys
-  const int n_iter = num_qb - qb0;
+  int n_iter = num_qb - qb0;
   const int col_q = head * 3 * D, col_k = col_q + D, col_v = col_q + 2 * D;
   const int krow0 = batch * args.S + jb * ATT_BN;
 
@@ -348,6 +370,20 @@ __global__ void __launch_bounds__(kAttThreads, 1)
   }
   __syncthreads();
   pdl_wait();  // prologue above overlapped the predecessor; Q/K/V, dO, lse, delta are read below
+  if constexpr (SEG) {
+    // the last query that sees a key of this block ends the document holding its last key: the first q > k_last with
+    // seg_start[q] > k_last, found by binary search over the row's non-decreasing seg_start.  Every thread computes the
+    // same count, so the producer and the consumers agree on it.
+    const int* seg_row = args.seg_start + static_cast<size_t>(batch) * args.S;
+    const int k_last = min(jb * ATT_BN + ATT_BN - 1, args.S - 1);
+    int lo = k_last + 1, hi = args.S;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (seg_row[mid] > k_last) hi = mid;
+      else lo = mid + 1;
+    }
+    n_iter = (lo + ATT_BWD_BM - 1) / ATT_BWD_BM - qb0;
+  }
 
   if (warp < 4) {
     setmaxnreg_dec<kAttRegsLight>();
@@ -440,11 +476,14 @@ __global__ void __launch_bounds__(kAttThreads, 1)
         const size_t stat_idx = (static_cast<size_t>(batch) * args.H + head) * args.S + qpos;
         const float lse2 = q_ok ? args.lse[stat_idx] * kLog2e : 0.f;
         const float nds = q_ok ? -args.delta[stat_idx] * args.scale : 0.f;
+        int seg_q = 0;
+        if constexpr (SEG) seg_q = q_ok ? args.seg_start[static_cast<size_t>(batch) * args.S + qpos] : 0;
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
           const int i = 4 * jn + 2 * hh + e;
           float p = fast_exp2(fmaf(st[i], args.scale_log2, fmaf(slope2, static_cast<float>(kpos[hh] - qpos), -lse2)));
           if (!q_ok || kpos[hh] > qpos) p = 0.f;
+          if (SEG && kpos[hh] < seg_q) p = 0.f;
           st[i] = p;
           dpt[i] = p * fmaf(dpt[i], args.scale, nds);
         }
@@ -584,24 +623,25 @@ static int att_tmap(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t c
     }                                                                               \
   } while (0)
 
-template <int D>
+template <int D, bool SEG>
 static int launch_att_fwd(const CUtensorMap& tm, const AttFwdArgs& a, cudaStream_t s) {
   using Cfg = AttFwdCfg<D>;
   static bool set = false;
   if (!set) {
-    if (cudaFuncSetAttribute(attention_fwd_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) != cudaSuccess) return -1;
+    if (cudaFuncSetAttribute(attention_fwd_kernel<D, SEG>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) != cudaSuccess) return -1;
     set = true;
   }
   dim3 grid((a.S + ATT_BM - 1) / ATT_BM, a.H, a.B);
-  if (launch_pdl(attention_fwd_kernel<D>, grid, dim3(kAttThreads), Cfg::kSmemBytes, s, tm, a) != cudaSuccess) return -1;
+  if (launch_pdl(attention_fwd_kernel<D, SEG>, grid, dim3(kAttThreads), Cfg::kSmemBytes, s, tm, a) != cudaSuccess) return -1;
   PG_CHECK_LAUNCH("attention_fwd");
   return 0;
 }
 
 // softmax_scale <= 0: 1/sqrt(D).  An explicit scale lets a head that was zero-padded to a supported width (e.g. D=80
 // -> 128: the padded columns contribute nothing to Q.K) keep the scale of its true width.
+// seg_start: int32 [B*S] row-relative document starts (packed sequences), nullptr: one document per row.
 extern "C" int pg_attention_fwd(const void* qkv, const float* slopes, void* out, float* lse, int B, int S, int H,
-                                int D, float softmax_scale, cudaStream_t s) {
+                                int D, float softmax_scale, const int* seg_start, cudaStream_t s) {
   if (D != 64 && D != 128) return -1;
   CUtensorMap tm;
   if (att_tmap(&tm, qkv, static_cast<uint64_t>(B) * S, static_cast<uint64_t>(H) * 3 * D, ATT_BM) != 0) return -1;
@@ -612,20 +652,22 @@ extern "C" int pg_attention_fwd(const void* qkv, const float* slopes, void* out,
   a.B = B; a.S = S; a.H = H;
   a.ld_out = H * D;
   a.scale_log2 = kLog2e * (softmax_scale > 0.f ? softmax_scale : 1.0f / sqrtf(static_cast<float>(D)));
-  return D == 64 ? launch_att_fwd<64>(tm, a, s) : launch_att_fwd<128>(tm, a, s);
+  a.seg_start = seg_start;
+  if (seg_start != nullptr) return D == 64 ? launch_att_fwd<64, true>(tm, a, s) : launch_att_fwd<128, true>(tm, a, s);
+  return D == 64 ? launch_att_fwd<64, false>(tm, a, s) : launch_att_fwd<128, false>(tm, a, s);
 }
 
-template <int D>
+template <int D, bool SEG>
 static int launch_att_bwd(const CUtensorMap& tkv, const CUtensorMap& tq, const CUtensorMap& tdo, const AttBwdArgs& a,
                           cudaStream_t s) {
   using Cfg = AttBwdCfg<D>;
   static bool set = false;
   if (!set) {
-    if (cudaFuncSetAttribute(attention_bwd_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) != cudaSuccess) return -1;
+    if (cudaFuncSetAttribute(attention_bwd_kernel<D, SEG>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) != cudaSuccess) return -1;
     set = true;
   }
   dim3 grid((a.S + ATT_BN - 1) / ATT_BN, a.H, a.B);
-  if (launch_pdl(attention_bwd_kernel<D>, grid, dim3(kAttThreads), Cfg::kSmemBytes, s, tkv, tq, tdo, a) != cudaSuccess) return -1;
+  if (launch_pdl(attention_bwd_kernel<D, SEG>, grid, dim3(kAttThreads), Cfg::kSmemBytes, s, tkv, tq, tdo, a) != cudaSuccess) return -1;
   PG_CHECK_LAUNCH("attention_bwd");
   return 0;
 }
@@ -633,7 +675,7 @@ static int launch_att_bwd(const CUtensorMap& tkv, const CUtensorMap& tq, const C
 // dq_acc: fp32 workspace [B*S, H*D]; delta: fp32 [B, H, S]
 extern "C" int pg_attention_bwd(const void* qkv, const float* slopes, const void* out, const float* lse,
                                 const void* dout, void* dqkv, float* dq_acc, float* delta, int B, int S, int H,
-                                int D, float softmax_scale, cudaStream_t s) {
+                                int D, float softmax_scale, const int* seg_start, cudaStream_t s) {
   if (D != 64 && D != 128) return -1;
   const int64_t rows = static_cast<int64_t>(B) * S;
   CUtensorMap tkv, tq, tdo;
@@ -652,7 +694,10 @@ extern "C" int pg_attention_bwd(const void* qkv, const float* slopes, const void
   a.B = B; a.S = S; a.H = H;
   a.scale = softmax_scale > 0.f ? softmax_scale : 1.0f / sqrtf(static_cast<float>(D));
   a.scale_log2 = a.scale * kLog2e;
-  const int rc = D == 64 ? launch_att_bwd<64>(tkv, tq, tdo, a, s) : launch_att_bwd<128>(tkv, tq, tdo, a, s);
+  a.seg_start = seg_start;
+  const int rc = seg_start != nullptr
+                     ? (D == 64 ? launch_att_bwd<64, true>(tkv, tq, tdo, a, s) : launch_att_bwd<128, true>(tkv, tq, tdo, a, s))
+                     : (D == 64 ? launch_att_bwd<64, false>(tkv, tq, tdo, a, s) : launch_att_bwd<128, false>(tkv, tq, tdo, a, s));
   if (rc != 0) return rc;
   const int64_t total = rows * H * D;
   if (launch_pdl(attention_dq_convert_kernel, dim3((unsigned)((total / 8 + 255) / 256)), dim3(256), 0, s, (const float*)dq_acc,

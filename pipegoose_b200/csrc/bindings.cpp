@@ -303,24 +303,38 @@ void grad_rs_accum(const torch::Tensor& src, torch::Tensor dst, double scale, co
                                &grs, cur_stream()) == 0, "grad_rs_accum failed");
 }
 
+// seg_start: optional int32 [B*S] row-relative document starts of packed sequences (see attention_sm90.cu)
+const int* seg_start_ptr(const c10::optional<torch::Tensor>& seg_start, const torch::Tensor& qkv, int64_t B, int64_t S) {
+  if (!seg_start.has_value()) return nullptr;
+  const torch::Tensor& t = *seg_start;
+  TORCH_CHECK(t.is_cuda() && t.device() == qkv.device(), "seg_start must be on the device of qkv");
+  TORCH_CHECK(t.scalar_type() == torch::kInt32, "seg_start must be int32");
+  TORCH_CHECK(t.is_contiguous(), "seg_start must be contiguous");
+  TORCH_CHECK(t.numel() == B * S, "seg_start must hold B*S = ", B * S, " entries, got ", t.numel());
+  return t.data_ptr<int>();
+}
+
 void attention_fwd(const torch::Tensor& qkv, const torch::Tensor& slopes, torch::Tensor out, torch::Tensor lse,
-                   int64_t B, int64_t S, int64_t H, int64_t D, double softmax_scale) {
+                   int64_t B, int64_t S, int64_t H, int64_t D, double softmax_scale,
+                   const c10::optional<torch::Tensor>& seg_start) {
   PG_CUDA(qkv); PG_BF16(qkv); PG_CUDA(out); PG_BF16(out); PG_CUDA(slopes); PG_F32(slopes); PG_CUDA(lse); PG_F32(lse);
   c10::cuda::CUDAGuard guard(qkv.device());
   TORCH_CHECK(qkv.numel() == B * S * H * 3 * D && out.numel() == B * S * H * D && lse.numel() == B * H * S && slopes.numel() == H, "attention_fwd: shape mismatch");
-  TORCH_CHECK(pg_attention_fwd(qkv.data_ptr(), slopes.data_ptr<float>(), out.data_ptr(), lse.data_ptr<float>(), (int)B, (int)S, (int)H, (int)D, (float)softmax_scale, cur_stream()) == 0, "attention_fwd failed");
+  const int* seg = seg_start_ptr(seg_start, qkv, B, S);
+  TORCH_CHECK(pg_attention_fwd(qkv.data_ptr(), slopes.data_ptr<float>(), out.data_ptr(), lse.data_ptr<float>(), (int)B, (int)S, (int)H, (int)D, (float)softmax_scale, seg, cur_stream()) == 0, "attention_fwd failed");
 }
 
 void attention_bwd(const torch::Tensor& qkv, const torch::Tensor& slopes, const torch::Tensor& out, const torch::Tensor& lse,
                    const torch::Tensor& dout, torch::Tensor dqkv, int64_t B, int64_t S, int64_t H, int64_t D,
-                   double softmax_scale) {
+                   double softmax_scale, const c10::optional<torch::Tensor>& seg_start) {
   PG_CUDA(qkv); PG_BF16(qkv); PG_CUDA(out); PG_BF16(out); PG_CUDA(dout); PG_BF16(dout); PG_CUDA(dqkv); PG_BF16(dqkv); PG_CUDA(lse); PG_F32(lse);
   c10::cuda::CUDAGuard guard(qkv.device());
   TORCH_CHECK(dout.numel() == out.numel() && dqkv.numel() == qkv.numel(), "attention_bwd: shape mismatch");
+  const int* seg = seg_start_ptr(seg_start, qkv, B, S);
   auto dq_acc = torch::empty({B * S, H * D}, qkv.options().dtype(torch::kFloat32));
   auto delta = torch::empty({B, H, S}, qkv.options().dtype(torch::kFloat32));
   TORCH_CHECK(pg_attention_bwd(qkv.data_ptr(), slopes.data_ptr<float>(), out.data_ptr(), lse.data_ptr<float>(), dout.data_ptr(), dqkv.data_ptr(),
-                               dq_acc.data_ptr<float>(), delta.data_ptr<float>(), (int)B, (int)S, (int)H, (int)D, (float)softmax_scale, cur_stream()) == 0, "attention_bwd failed");
+                               dq_acc.data_ptr<float>(), delta.data_ptr<float>(), (int)B, (int)S, (int)H, (int)D, (float)softmax_scale, seg, cur_stream()) == 0, "attention_bwd failed");
 }
 
 void moe_route(const torch::Tensor& x, const torch::Tensor& wg, const c10::optional<torch::Tensor>& bg,
@@ -492,9 +506,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sgd_step", &sgd_step);
   m.def("accum_bf16_to_f32", &accum_bf16_to_f32);
   m.def("attention_fwd", &attention_fwd, py::arg("qkv"), py::arg("slopes"), py::arg("out"), py::arg("lse"), py::arg("B"),
-        py::arg("S"), py::arg("H"), py::arg("D"), py::arg("softmax_scale") = 0.0);
+        py::arg("S"), py::arg("H"), py::arg("D"), py::arg("softmax_scale") = 0.0, py::arg("seg_start") = py::none());
   m.def("attention_bwd", &attention_bwd, py::arg("qkv"), py::arg("slopes"), py::arg("out"), py::arg("lse"), py::arg("dout"),
-        py::arg("dqkv"), py::arg("B"), py::arg("S"), py::arg("H"), py::arg("D"), py::arg("softmax_scale") = 0.0);
+        py::arg("dqkv"), py::arg("B"), py::arg("S"), py::arg("H"), py::arg("D"), py::arg("softmax_scale") = 0.0,
+        py::arg("seg_start") = py::none());
   m.def("moe_route", &moe_route);
   m.def("moe_dispatch", &moe_dispatch);
   m.def("symm_alloc", &symm_alloc);

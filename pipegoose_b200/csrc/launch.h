@@ -74,11 +74,12 @@ typedef struct PgGemmDesc {
 } PgGemmDesc;
 
 // ---- attention_sm90.cu
+// seg_start: int32 [B*S] row-relative document starts of packed sequences (nullptr: one document per row)
 int pg_attention_fwd(const void* qkv, const float* slopes, void* out, float* lse, int B, int S, int H, int D,
-                     float softmax_scale, cudaStream_t s);
+                     float softmax_scale, const int* seg_start, cudaStream_t s);
 int pg_attention_bwd(const void* qkv, const float* slopes, const void* out, const float* lse, const void* dout,
                      void* dqkv, float* dq_acc, float* delta, int B, int S, int H, int D, float softmax_scale,
-                     cudaStream_t s);
+                     const int* seg_start, cudaStream_t s);
 
 // ---- moe.cu
 int pg_moe_route(const void* x, const void* wg, const void* bg, const float* jitter, int n, int h, int E, int top_k,

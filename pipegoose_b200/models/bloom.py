@@ -146,7 +146,8 @@ class BloomBlock(nn.Module):
         self.hidden_dropout = float(getattr(config, "hidden_dropout", 0.0))
         self.tp = None  # set by TensorParallel (sequence-parallel communicator)
 
-    def _forward_with_dropout(self, x: torch.Tensor, batch: int, seq: int) -> torch.Tensor:
+    def _forward_with_dropout(self, x: torch.Tensor, batch: int, seq: int,
+                              seg_start: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``hidden_dropout > 0`` or ``attention_dropout > 0`` in training: ``x + dropout(dense(attention))`` and
         ``x + dropout(mlp)`` — the kernels of the fused path with the residual add applied after the dropout instead of
         in the GEMM epilogue; attention probabilities are dropped in ``alibi_attention_with_dropout``."""
@@ -160,7 +161,7 @@ class BloomBlock(nn.Module):
         qkv = PF.layernorm_linear(x, self.input_layernorm.weight, self.input_layernorm.bias,
                                   attn.query_key_value.weight, attn.query_key_value.bias, self.eps, tp)
         att = alibi_attention(qkv, attn.alibi_slopes_local(n_head_local), batch, seq, n_head_local, attn.head_dim,
-                              dropout_p=getattr(self, "attention_dropout", 0.0))
+                              dropout_p=getattr(self, "attention_dropout", 0.0), seg_start=seg_start)
         x = x + F.dropout(PF.linear_residual(att, attn.dense.weight, attn.dense.bias, zero, tp), p, True)
         mlp = self.mlp
         if isinstance(mlp, BloomMLP):
@@ -170,17 +171,19 @@ class BloomBlock(nn.Module):
         ln = fused_layer_norm(x, self.post_attention_layernorm.weight, self.post_attention_layernorm.bias, self.eps)
         return x + F.dropout(mlp(ln, zero), p, True)
 
-    def forward(self, x: torch.Tensor, batch: int, seq: int) -> torch.Tensor:
-        """``x``: ``[tokens_local, hidden]`` (token-sharded when ``self.tp`` is set)."""
+    def forward(self, x: torch.Tensor, batch: int, seq: int, seg_start: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``x``: ``[tokens_local, hidden]`` (token-sharded when ``self.tp`` is set).  ``seg_start``: int32 ``[batch, seq]``
+        document starts of packed rows (``ops.attention``), the same on every tensor-parallel rank; None: one document
+        per row."""
         if self.training and (getattr(self, "hidden_dropout", 0.0) > 0.0 or getattr(self, "attention_dropout", 0.0) > 0.0):
-            return self._forward_with_dropout(x, batch, seq)
+            return self._forward_with_dropout(x, batch, seq, seg_start)
         attn = self.self_attention
         tp = self.tp
         n_head_local = attn.query_key_value.weight.shape[0] // (3 * attn.head_dim)
         x = PF.attention_sublayer(x, self.input_layernorm.weight, self.input_layernorm.bias,
                                   attn.query_key_value.weight, attn.query_key_value.bias,
                                   attn.dense.weight, attn.dense.bias, attn.alibi_slopes_local(n_head_local),
-                                  self.eps, batch, seq, n_head_local, attn.head_dim, tp)
+                                  self.eps, batch, seq, n_head_local, attn.head_dim, tp, seg_start)
         mlp = self.mlp
         if isinstance(mlp, BloomMLP):
             x = PF.layernorm_mlp(x, self.post_attention_layernorm.weight, self.post_attention_layernorm.bias,
@@ -253,10 +256,34 @@ def left_align(attention_mask: torch.Tensor):
     return idx, keep, (pos - lead) % S
 
 
-def embed_tokens(owner: nn.Module, input_ids: torch.Tensor, config, vocab_start: int, tp) -> torch.Tensor:
+def validate_position_ids(position_ids: torch.Tensor, input_ids: torch.Tensor) -> None:
+    """Packed-sequence positions: ``[B, S]`` like ``input_ids``, every row a concatenation of runs ``0, 1, 2, ...``
+    (``P[:, 0] == 0``, every step ``+1`` or a reset to 0).  The values are checked with a device-side assert — no host
+    sync."""
+    if tuple(position_ids.shape) != tuple(input_ids.shape):
+        raise ValueError(f"position_ids has shape {tuple(position_ids.shape)}, input_ids {tuple(input_ids.shape)}")
+    if position_ids.dtype.is_floating_point or position_ids.dtype == torch.bool:
+        raise ValueError(f"position_ids must be an integer tensor, got {position_ids.dtype}")
+    P = position_ids
+    step = P[:, 1:] - P[:, :-1]
+    ok = (P[:, 0] == 0).all() & ((step == 1) | (P[:, 1:] == 0)).all()
+    torch._assert_async(ok, "position_ids rows must be runs 0, 1, 2, ... (start at 0; each step +1 or a reset to 0)")
+
+
+def packed_seg_start(position_ids: torch.Tensor, input_ids: torch.Tensor) -> torch.Tensor:
+    """Validated ``position_ids`` -> int32 ``[B, S]`` document starts for the attention kernels."""
+    from pipegoose_b200.ops.attention import seg_start_from_position_ids
+
+    validate_position_ids(position_ids, input_ids)
+    return seg_start_from_position_ids(position_ids.to(input_ids.device))
+
+
+def embed_tokens(owner: nn.Module, input_ids: torch.Tensor, config, vocab_start: int, tp,
+                 position_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Token ids -> ``[tokens_local, hidden]`` input of the first block.  ``owner`` holds ``word_embeddings`` and either
     ``word_embeddings_layernorm`` (Bloom) or ``position_embeddings`` (GPT-2): the model's ``transformer`` or a first
-    pipeline stage."""
+    pipeline stage.  ``position_ids`` (packed rows): the positions learned position embeddings read instead of
+    ``arange(S)``; ALiBi models take no positions here."""
     if tp is not None and input_ids.numel() % tp.size != 0:
         raise ValueError(f"the sequence-parallel path shards the {input_ids.numel()} tokens of a batch (batch x seq) over "
                          f"{tp.size} tensor-parallel ranks: pad the batch so that batch x seq is a multiple of {tp.size}")
@@ -264,19 +291,22 @@ def embed_tokens(owner: nn.Module, input_ids: torch.Tensor, config, vocab_start:
         assert input_ids.shape[-1] <= config.n_positions, "sequence longer than the position table"
         assert not getattr(config, "embedding_layernorm", False)
         return PF.embedding_positions(input_ids, owner.word_embeddings.weight, owner.position_embeddings.weight,
-                                      vocab_start, tp)
+                                      vocab_start, tp, position_ids)
     ln = owner.word_embeddings_layernorm
     return PF.embedding_layernorm(input_ids, owner.word_embeddings.weight, ln.weight, ln.bias,
                                   config.layer_norm_epsilon, vocab_start, tp)
 
 
-def run_block(block: nn.Module, x: torch.Tensor, batch: int, seq: int, config) -> torch.Tensor:
-    """One transformer block, with activation recomputation when ``config.recompute == "block"`` (training only)."""
+def run_block(block: nn.Module, x: torch.Tensor, batch: int, seq: int, config,
+              seg_start: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """One transformer block, with activation recomputation when ``config.recompute == "block"`` (training only).
+    ``seg_start``: document starts of packed rows (see :meth:`BloomBlock.forward`)."""
+    args = (x, batch, seq) if seg_start is None else (x, batch, seq, seg_start)
     if getattr(config, "recompute", "none") == "block" and torch.is_grad_enabled() and x.requires_grad:
         from torch.utils.checkpoint import checkpoint
 
-        return checkpoint(block, x, batch, seq, use_reentrant=False)
-    return block(x, batch, seq)
+        return checkpoint(block, *args, use_reentrant=False)
+    return block(*args)
 
 
 class BloomModel(nn.Module):
@@ -347,19 +377,39 @@ class BloomForCausalLM(nn.Module):
         return 3 * 2 * (L * (per_layer + attn) + V * h)
 
     # ------------------------------------------------------------------ forward
-    def hidden_states(self, input_ids: torch.Tensor) -> torch.Tensor:
+    def hidden_states(self, input_ids: torch.Tensor, position_ids: Optional[torch.Tensor] = None,
+                      seg_start: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``position_ids``: packed rows (see :meth:`forward`); ``seg_start``: their document starts when the caller
+        already derived them (:func:`packed_seg_start`)."""
         t = self.transformer
         B, S = input_ids.shape
-        x = embed_tokens(t, input_ids, self.config, self.vocab_start, self.tp)
+        if position_ids is not None and seg_start is None:
+            seg_start = packed_seg_start(position_ids, input_ids)
+        x = embed_tokens(t, input_ids, self.config, self.vocab_start, self.tp, position_ids)
         for block in t.h:
-            x = run_block(block, x, B, S, self.config)
+            x = run_block(block, x, B, S, self.config, seg_start)
         return x
 
     def forward(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,
-                labels: Optional[torch.Tensor] = None, **_unused) -> CausalLMOutput:
+                labels: Optional[torch.Tensor] = None, position_ids: Optional[torch.Tensor] = None,
+                **_unused) -> CausalLMOutput:
+        """``position_ids`` (``[B, S]``, packed sequences, as 🤗's ``DataCollatorWithFlattening`` emits them): every row
+        is a concatenation of documents, each numbered ``0, 1, 2, ...``.  Tokens attend only within their document,
+        learned position embeddings read these positions, and a document's last token has no target (the next
+        document's first token is not predicted).  The result equals running every document as its own sequence, with
+        the loss averaged over all documents' target tokens.  Not combined with an ``attention_mask`` that has zeros:
+        pad the tail of a packed row as one more document with ``-100`` labels instead."""
         t = self.transformer
         B, S = input_ids.shape
         unroll = None
+        seg_start = None
+        if position_ids is not None:
+            if attention_mask is not None and bool((attention_mask == 0).any()):
+                raise ValueError("position_ids (packed sequences) cannot be combined with an attention_mask that has "
+                                 "zeros: pad the tail of a packed row as one more document with -100 labels instead")
+            attention_mask = None
+            position_ids = position_ids.to(input_ids.device)
+            seg_start = packed_seg_start(position_ids, input_ids)
         if attention_mask is not None:
             # The fused attention is purely causal.  RIGHT padding is harmless under a causal mask (real tokens never
             # attend to later pads).  LEFT padding (what 🤗's Bloom tokenizer produces) is turned into right padding by
@@ -369,12 +419,14 @@ class BloomForCausalLM(nn.Module):
             input_ids = input_ids.gather(1, idx)
             if labels is not None:
                 labels = labels.gather(1, idx).masked_fill(~keep, -100)
-        x = self.hidden_states(input_ids)
+        x = self.hidden_states(input_ids, position_ids, seg_start)
         eps = self.config.layer_norm_epsilon
         if labels is not None:
             # HF semantics: position s predicts token s+1; the last position has no target
             shifted = torch.full_like(labels, -100)
             shifted[:, :-1] = labels[:, 1:]
+            if position_ids is not None:   # nor does the last token of a packed document
+                shifted[:, :-1].masked_fill_(position_ids[:, 1:] == 0, -100)
             loss = PF.lm_head_cross_entropy(x, t.ln_f.weight, t.ln_f.bias, self.lm_head.weight, shifted, eps,
                                             self.vocab_start, -100, self.tp, vocab_size=self.config.vocab_size)
             return CausalLMOutput(loss=loss, logits=None)

@@ -79,6 +79,9 @@ class JobPipelineEngine:
     def run(self, input_ids=None, attention_mask=None, labels=None, **kwargs):
         from pipegoose_b200.models.bloom import CausalLMOutput
 
+        if kwargs.get("position_ids") is not None:
+            raise ValueError("PipelineParallel does not take position_ids (packed sequences): micro-batches are cut from "
+                             "whole rows without them; train packed batches without pipeline parallelism")
         assert labels is not None, "the job runtime engine implements the training step (pass labels)"
         ctx = self.parallel_context
         me = ctx.get_global_rank()

@@ -538,6 +538,9 @@ class PipelineEngine:
         """``loss_scale`` (keyword): factor on this call's gradients — pass ``1 / k`` on each of the ``k`` calls of a
         gradient-accumulation step (the backward pass runs inside this call, a later ``(loss / k).backward()`` cannot
         scale it any more).  The returned loss is unscaled."""
+        if kwargs.get("position_ids") is not None:
+            raise ValueError("PipelineParallel does not take position_ids (packed sequences): micro-batches are cut from "
+                             "whole rows without them; train packed batches without pipeline parallelism")
         inputs = {"input_ids": input_ids, "attention_mask": attention_mask, "labels": labels}
         inputs.update(kwargs)
         if labels is None:

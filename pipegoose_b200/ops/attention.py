@@ -7,6 +7,10 @@
 Two implementations share this contract: the sm_90a flash kernel (``csrc/attention_sm90.cu``:
 wgmma QK^T / PV with register accumulators, online softmax, never materialising ``[S, S]``) and
 the PyTorch reference below (CPU tests, numerics oracle).
+
+Packed sequences: ``seg_start`` (int32 ``[B, S]`` or ``[B*S]``, see :func:`seg_start_from_position_ids`) holds, for
+every token, the row-relative position where its document begins.  Query ``q`` then sees key ``k`` iff
+``seg_start[q] <= k <= q``: documents packed into one row do not attend to each other.  ``None``: one document per row.
 """
 from __future__ import annotations
 
@@ -17,17 +21,35 @@ import torch
 from pipegoose_b200.ops import has_kernel, native, use_native
 
 
+def seg_start_from_position_ids(position_ids: torch.Tensor) -> torch.Tensor:
+    """int32 ``[B, S]`` document starts of packed rows: ``seg_start[b, s] = s - position_ids[b, s]``, where every row of
+    ``position_ids`` is a concatenation of runs ``0, 1, 2, ...`` (one per document).  Nothing is checked here; the models
+    validate ``position_ids`` on the device first."""
+    S = position_ids.shape[-1]
+    pos = torch.arange(S, device=position_ids.device, dtype=position_ids.dtype)
+    return (pos - position_ids).to(torch.int32).contiguous()
+
+
+def visible_mask(S: int, device, seg_start=None, B: int = 1) -> torch.Tensor:
+    """Boolean visibility of key ``k`` from query ``q``: ``[S, S]`` causal, or ``[B, 1, S, S]`` with the document lower
+    bound ``k >= seg_start[b, q]`` of packed rows."""
+    causal = torch.ones(S, S, dtype=torch.bool, device=device).tril()
+    if seg_start is None:
+        return causal
+    k = torch.arange(S, device=device)
+    return causal & (k.view(1, 1, 1, S) >= seg_start.reshape(B, 1, S, 1).to(device))
+
+
 def alibi_attention_reference(qkv: torch.Tensor, slopes: torch.Tensor, B: int, S: int, n_head: int, D: int,
-                              softmax_scale: float = 0.0, dropout_p: float = 0.0) -> torch.Tensor:
+                              softmax_scale: float = 0.0, dropout_p: float = 0.0, seg_start=None) -> torch.Tensor:
     """``dropout_p > 0``: dropout on the attention probabilities (🤗 Bloom's ``attention_dropout``: zeroed entries, the
-    rest scaled by ``1 / (1 - p)``, rows not re-normalised)."""
+    rest scaled by ``1 / (1 - p)``, rows not re-normalised).  ``seg_start``: packed documents (module docstring)."""
     x = qkv.view(B, S, n_head, 3, D)
     q, k, v = (x[:, :, :, i].permute(0, 2, 1, 3).float() for i in range(3))  # [B, H, S, D]
     scores = torch.matmul(q, k.transpose(-1, -2)) * (softmax_scale if softmax_scale > 0 else 1.0 / math.sqrt(D))
     pos = torch.arange(S, device=qkv.device, dtype=torch.float32)
     scores = scores + slopes.float().view(1, n_head, 1, 1) * pos.view(1, 1, 1, S)
-    causal = torch.ones(S, S, dtype=torch.bool, device=qkv.device).tril()
-    scores = scores.masked_fill(~causal, float("-inf"))
+    scores = scores.masked_fill(~visible_mask(S, qkv.device, seg_start, B), float("-inf"))
     p = torch.softmax(scores, dim=-1)
     if dropout_p > 0.0:
         p = torch.nn.functional.dropout(p, dropout_p, True)
@@ -36,14 +58,14 @@ def alibi_attention_reference(qkv: torch.Tensor, slopes: torch.Tensor, B: int, S
 
 
 def alibi_attention_with_dropout(qkv: torch.Tensor, slopes: torch.Tensor, B: int, S: int, n_head: int, D: int,
-                                 dropout_p: float) -> torch.Tensor:
+                                 dropout_p: float, seg_start=None) -> torch.Tensor:
     """Training-time attention with dropout on the probabilities.  The flash kernel never holds a row of probabilities
     (online softmax), so this path materialises them: bf16 GEMMs around an fp32 softmax, one head group at a time so
     that the live ``[B, heads, S, S]`` block stays below ~1 GiB whatever the model.  Differentiated by autograd."""
     x = qkv.view(B, S, n_head, 3, D)
     scale = 1.0 / math.sqrt(D)
     pos = torch.arange(S, device=qkv.device, dtype=torch.float32)
-    causal = torch.ones(S, S, dtype=torch.bool, device=qkv.device).tril()
+    hidden = ~visible_mask(S, qkv.device, seg_start, B)
     group = max(1, min(n_head, (1 << 28) // max(1, B * S * S)))     # heads per block: <= 2^28 fp32 scores
     outs = []
     for h0 in range(0, n_head, group):
@@ -51,30 +73,36 @@ def alibi_attention_with_dropout(qkv: torch.Tensor, slopes: torch.Tensor, B: int
         q, k, v = (x[:, :, h0:h1, i].permute(0, 2, 1, 3) for i in range(3))      # [B, g, S, D] views
         scores = torch.matmul(q, k.transpose(-1, -2)).float() * scale
         scores = scores + slopes[h0:h1].float().view(1, -1, 1, 1) * pos.view(1, 1, 1, S)
-        p = torch.softmax(scores.masked_fill(~causal, float("-inf")), dim=-1)
+        p = torch.softmax(scores.masked_fill(hidden, float("-inf")), dim=-1)
         p = torch.nn.functional.dropout(p, dropout_p, True).to(qkv.dtype)
         outs.append(torch.matmul(p, v))
     out = outs[0] if len(outs) == 1 else torch.cat(outs, dim=1)
     return out.permute(0, 2, 1, 3).reshape(B * S, n_head * D)
 
 
+def native_seg_start(seg_start):
+    """``seg_start`` as the flash kernels take it: contiguous int32 ``[B*S]`` (None stays None)."""
+    return None if seg_start is None else seg_start.reshape(-1).to(torch.int32).contiguous()
+
+
 class _AlibiAttentionNative(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, qkv, slopes, B, S, n_head, D):
+    def forward(ctx, qkv, slopes, B, S, n_head, D, seg_start=None):
         out = torch.empty(B * S, n_head * D, dtype=qkv.dtype, device=qkv.device)
         lse = torch.empty(B, n_head, S, dtype=torch.float32, device=qkv.device)
-        native().attention_fwd(qkv, slopes, out, lse, B, S, n_head, D)
-        ctx.save_for_backward(qkv, slopes, out, lse)
+        seg = native_seg_start(seg_start)
+        native().attention_fwd(qkv, slopes, out, lse, B, S, n_head, D, 0.0, seg)
+        ctx.save_for_backward(qkv, slopes, out, lse, seg)
         ctx.dims = (B, S, n_head, D)
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        qkv, slopes, out, lse = ctx.saved_tensors
+        qkv, slopes, out, lse, seg = ctx.saved_tensors
         B, S, n_head, D = ctx.dims
         dqkv = torch.empty_like(qkv)
-        native().attention_bwd(qkv, slopes, out, lse, dout.contiguous(), dqkv, B, S, n_head, D)
-        return dqkv, None, None, None, None, None
+        native().attention_bwd(qkv, slopes, out, lse, dout.contiguous(), dqkv, B, S, n_head, D, 0.0, seg)
+        return dqkv, None, None, None, None, None, None
 
 
 def _native_attention_available(D: int) -> bool:
@@ -109,43 +137,47 @@ class _AlibiAttentionPadded(torch.autograd.Function):
     columns add nothing to the scores, padded v columns produce output columns that are sliced away."""
 
     @staticmethod
-    def forward(ctx, qkv, slopes, B, S, n_head, D):
+    def forward(ctx, qkv, slopes, B, S, n_head, D, seg_start=None):
         DP = padded_head_dim(D)
         scale = 1.0 / math.sqrt(D)
         qkv_p = pad_heads(qkv, n_head, 3, D, DP).contiguous()
         out_p = torch.empty(B * S, n_head * DP, dtype=qkv.dtype, device=qkv.device)
         lse = torch.empty(B, n_head, S, dtype=torch.float32, device=qkv.device)
-        native().attention_fwd(qkv_p, slopes, out_p, lse, B, S, n_head, DP, scale)
-        ctx.save_for_backward(qkv_p, slopes, out_p, lse)
+        seg = native_seg_start(seg_start)
+        native().attention_fwd(qkv_p, slopes, out_p, lse, B, S, n_head, DP, scale, seg)
+        ctx.save_for_backward(qkv_p, slopes, out_p, lse, seg)
         ctx.dims = (B, S, n_head, D, DP, scale)
         return unpad_heads(out_p, n_head, 1, D, DP).contiguous()
 
     @staticmethod
     def backward(ctx, dout):
-        qkv_p, slopes, out_p, lse = ctx.saved_tensors
+        qkv_p, slopes, out_p, lse, seg = ctx.saved_tensors
         B, S, n_head, D, DP, scale = ctx.dims
         dout_p = pad_heads(dout.contiguous(), n_head, 1, D, DP).contiguous()
         dqkv_p = torch.empty_like(qkv_p)
-        native().attention_bwd(qkv_p, slopes, out_p, lse, dout_p, dqkv_p, B, S, n_head, DP, scale)
-        return unpad_heads(dqkv_p, n_head, 3, D, DP).contiguous(), None, None, None, None, None
+        native().attention_bwd(qkv_p, slopes, out_p, lse, dout_p, dqkv_p, B, S, n_head, DP, scale, seg)
+        return unpad_heads(dqkv_p, n_head, 3, D, DP).contiguous(), None, None, None, None, None, None
 
 
 def alibi_attention(qkv: torch.Tensor, slopes: torch.Tensor, B: int, S: int, n_head: int, D: int,
-                    dropout_p: float = 0.0) -> torch.Tensor:
+                    dropout_p: float = 0.0, seg_start=None) -> torch.Tensor:
+    """``seg_start``: document starts of packed rows (module docstring), ``None``: one document per row."""
     if dropout_p > 0.0:
-        return alibi_attention_with_dropout(qkv, slopes, B, S, n_head, D, dropout_p)
+        return alibi_attention_with_dropout(qkv, slopes, B, S, n_head, D, dropout_p, seg_start=seg_start)
     if use_native(qkv) and _native_attention_available(D):
-        return _AlibiAttentionNative.apply(qkv, slopes, B, S, n_head, D)
+        return _AlibiAttentionNative.apply(qkv, slopes, B, S, n_head, D, seg_start)
     if use_native(qkv) and has_kernel("attention_fwd") and padded_head_dim(D) > 0 and D % 8 == 0:
-        return _AlibiAttentionPadded.apply(qkv, slopes, B, S, n_head, D)  # e.g. D=80 (bloom-3b) on the D=128 kernel
+        # e.g. D=80 (bloom-3b) on the D=128 kernel
+        return _AlibiAttentionPadded.apply(qkv, slopes, B, S, n_head, D, seg_start)
     if qkv.is_cuda:
         # library fallback for head sizes beyond the kernel's widest tile (D > 128)
         x = qkv.view(B, S, n_head, 3, D)
         q, k, v = (x[:, :, :, i].permute(0, 2, 1, 3) for i in range(3))
         pos = torch.arange(S, device=qkv.device, dtype=torch.float32)
         bias = slopes.float().view(1, n_head, 1, 1) * pos.view(1, 1, 1, S)
-        causal = torch.ones(S, S, dtype=torch.bool, device=qkv.device).tril()
-        bias = bias.expand(1, n_head, S, S).masked_fill(~causal, float("-inf")).to(qkv.dtype)
+        visible = visible_mask(S, qkv.device, seg_start, B)
+        rows = 1 if seg_start is None else B
+        bias = bias.expand(rows, n_head, S, S).masked_fill(~visible, float("-inf")).to(qkv.dtype)
         out = torch.nn.functional.scaled_dot_product_attention(q, k, v, attn_mask=bias)
         return out.permute(0, 2, 1, 3).reshape(B * S, n_head * D)
-    return alibi_attention_reference(qkv, slopes, B, S, n_head, D)
+    return alibi_attention_reference(qkv, slopes, B, S, n_head, D, seg_start=seg_start)

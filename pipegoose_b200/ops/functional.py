@@ -197,15 +197,17 @@ class AttentionSubLayer(torch.autograd.Function):
     gradient is added inside the LN backward kernel instead of by an autograd accumulation pass."""
 
     @staticmethod
-    def forward(ctx, x, gamma, beta, wqkv, bqkv, wd, bd, slopes, eps, B, S, n_head, D, tp):
+    def forward(ctx, x, gamma, beta, wqkv, bqkv, wd, bd, slopes, eps, B, S, n_head, D, tp, seg_start=None):
         from pipegoose_b200.ops import native
+        from pipegoose_b200.ops.attention import native_seg_start
 
         qkv, mean, rstd, ln_full = _ln_linear_fwd(x, gamma, beta, wqkv, bqkv, eps, tp)
         att = torch.empty(B * S, n_head * D, dtype=qkv.dtype, device=qkv.device)
         lse = torch.empty(B, n_head, S, dtype=torch.float32, device=qkv.device)
-        native().attention_fwd(qkv, slopes, att, lse, B, S, n_head, D)
+        seg = native_seg_start(seg_start)
+        native().attention_fwd(qkv, slopes, att, lse, B, S, n_head, D, 0.0, seg)
         y = _linear_residual_fwd(att, wd, bd, x, tp)
-        ctx.save_for_backward(x, gamma, beta, wqkv, bqkv, wd, bd, slopes, mean, rstd, ln_full, qkv, att, lse)
+        ctx.save_for_backward(x, gamma, beta, wqkv, bqkv, wd, bd, slopes, mean, rstd, ln_full, qkv, att, lse, seg)
         ctx.tp = tp
         ctx.dims = (B, S, n_head, D)
         return y
@@ -214,16 +216,16 @@ class AttentionSubLayer(torch.autograd.Function):
     def backward(ctx, dy):
         from pipegoose_b200.ops import native
 
-        x, gamma, beta, wqkv, bqkv, wd, bd, slopes, mean, rstd, ln_full, qkv, att, lse = ctx.saved_tensors
+        x, gamma, beta, wqkv, bqkv, wd, bd, slopes, mean, rstd, ln_full, qkv, att, lse, seg = ctx.saved_tensors
         B, S, n_head, D = ctx.dims
         tp = ctx.tp
         dy = dy.contiguous()
         datt, dwd, dbd = _linear_residual_bwd(dy, att, wd, bd, tp)
         dqkv = torch.empty_like(qkv)
-        native().attention_bwd(qkv, slopes, att, lse, datt, dqkv, B, S, n_head, D)
+        native().attention_bwd(qkv, slopes, att, lse, datt, dqkv, B, S, n_head, D, 0.0, seg)
         dx, dgamma, dbeta, dwqkv, dbqkv = _ln_linear_bwd(dqkv, x, gamma, beta, wqkv, bqkv, mean, rstd, ln_full, tp,
                                                          dx_extra=dy)
-        return dx, dgamma, dbeta, dwqkv, dbqkv, dwd, dbd, None, None, None, None, None, None, None
+        return dx, dgamma, dbeta, dwqkv, dbqkv, dwd, dbd, None, None, None, None, None, None, None, None
 
 
 class LayerNormMLP(torch.autograd.Function):
@@ -386,10 +388,13 @@ class EmbeddingPositions(torch.autograd.Function):
     sequence-parallel aware: under TP every rank gathers the rows of its vocabulary slice for ALL tokens, the partial
     results are reduce-scattered over the token dimension, and the position rows of the LOCAL tokens are added.  The
     backward scatter-adds into the table's fp32 main grad like :class:`EmbeddingLayerNorm`; the position-table gradient
-    is a partial sum over this rank's tokens (the parameter is tagged ``tp_partial_grad``)."""
+    is a partial sum over this rank's tokens (the parameter is tagged ``tp_partial_grad``).
+
+    ``position_ids`` (``[B, S]``, packed sequences): the position of every token, flattened like the tokens; the local
+    rows' slice of it replaces ``arange(S)``."""
 
     @staticmethod
-    def forward(ctx, ids, table, positions, vocab_start, tp):
+    def forward(ctx, ids, table, positions, vocab_start, tp, position_ids=None):
         vocab_end = vocab_start + table.shape[0]
         flat = ids.reshape(-1)
         seq = ids.shape[-1]
@@ -399,7 +404,10 @@ class EmbeddingPositions(torch.autograd.Function):
         e = tp.reduce_scatter_rows(part.contiguous()) if tp is not None else part
         rows = e.shape[0]
         first = tp.rank * rows if tp is not None else 0
-        pos = (torch.arange(rows, device=e.device) + first) % seq
+        if position_ids is None:
+            pos = (torch.arange(rows, device=e.device) + first) % seq
+        else:
+            pos = position_ids.reshape(-1)[first:first + rows].to(device=e.device, dtype=torch.long)
         ctx.save_for_backward(flat, table, positions, pos)
         ctx.tp = tp
         ctx.vocab_start = vocab_start
@@ -425,7 +433,7 @@ class EmbeddingPositions(torch.autograd.Function):
         dtable = K.embedding_bwd(de_full, flat, table.shape[0], vocab_start, vocab_end, accum_into=mg)
         if mg is not None:
             notify_grad_ready(table)
-        return None, dtable, dpos, None, None
+        return None, dtable, dpos, None, None, None
 
 
 class LMHeadCrossEntropy(torch.autograd.Function):
@@ -501,15 +509,17 @@ def layernorm_linear(x, gamma, beta, weight, bias, eps=1e-5, tp=None):
     return LayerNormLinear.apply(x, gamma, beta, weight, bias, eps, tp)
 
 
-def attention_sublayer(x, gamma, beta, wqkv, bqkv, wd, bd, slopes, eps, B, S, n_head, D, tp=None):
-    """LN -> QKV -> causal ALiBi attention -> dense + residual (``x`` is the residual stream)."""
+def attention_sublayer(x, gamma, beta, wqkv, bqkv, wd, bd, slopes, eps, B, S, n_head, D, tp=None, seg_start=None):
+    """LN -> QKV -> causal ALiBi attention -> dense + residual (``x`` is the residual stream).  ``seg_start``: document
+    starts of packed rows (``ops.attention``), the same full-length tensor on every tensor-parallel rank: attention runs
+    on the all-gathered tokens."""
     from pipegoose_b200.ops import use_native
     from pipegoose_b200.ops.attention import _native_attention_available, alibi_attention
 
     if use_native(x, wqkv) and _native_attention_available(D):
-        return AttentionSubLayer.apply(x, gamma, beta, wqkv, bqkv, wd, bd, slopes, eps, B, S, n_head, D, tp)
+        return AttentionSubLayer.apply(x, gamma, beta, wqkv, bqkv, wd, bd, slopes, eps, B, S, n_head, D, tp, seg_start)
     qkv = LayerNormLinear.apply(x, gamma, beta, wqkv, bqkv, eps, tp)
-    att = alibi_attention(qkv, slopes, B, S, n_head, D)
+    att = alibi_attention(qkv, slopes, B, S, n_head, D, seg_start=seg_start)
     return LinearResidual.apply(att, wd, bd, x, tp)
 
 
@@ -529,8 +539,8 @@ def embedding_layernorm(ids, table, gamma, beta, eps=1e-5, vocab_start=0, tp=Non
     return EmbeddingLayerNorm.apply(ids, table, gamma, beta, eps, vocab_start, tp)
 
 
-def embedding_positions(ids, table, positions, vocab_start=0, tp=None):
-    return EmbeddingPositions.apply(ids, table, positions, vocab_start, tp)
+def embedding_positions(ids, table, positions, vocab_start=0, tp=None, position_ids=None):
+    return EmbeddingPositions.apply(ids, table, positions, vocab_start, tp, position_ids)
 
 
 def lm_head_cross_entropy(x, gamma, beta, table, labels, eps=1e-5, vocab_start=0, ignore_index=-100, tp=None,

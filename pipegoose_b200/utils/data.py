@@ -55,12 +55,20 @@ def build_dataloader(dataset, parallel_context, batch_size: int, shuffle: bool =
 class TokenFileDataset(Dataset):
     """Sequences of ``seq_len`` tokens over a flat file of token ids (``uint16`` / ``uint32`` / ``int64``, the layout
     ``write_token_file`` and most pre-tokenised corpora use).  Item ``i`` is tokens ``[i * stride, i * stride + seq_len)``
-    as ``{"input_ids": int64[seq_len]}`` (the models shift the labels themselves: pass ``labels=input_ids``)."""
+    as ``{"input_ids": int64[seq_len]}`` (the models shift the labels themselves: pass ``labels=input_ids``).
 
-    def __init__(self, path: str, seq_len: int, dtype: str = "uint16", stride: Optional[int] = None):
+    ``eos_token_id``: the file is a concatenation of documents, each ended by this token.  Every item then also carries
+    ``"position_ids"`` (int64 ``[seq_len]``): 0 at the window's first token, +1 per token, back to 0 on the token after
+    each ``eos_token_id`` (the eos belongs to the document it ends).  The models then keep the documents of a window
+    from attending to each other and from predicting each other's tokens; a ``Trainer`` passes the item to the model
+    as it is."""
+
+    def __init__(self, path: str, seq_len: int, dtype: str = "uint16", stride: Optional[int] = None,
+                 eos_token_id: Optional[int] = None):
         import numpy as np
 
         self.path, self.seq_len = path, int(seq_len)
+        self.eos_token_id = None if eos_token_id is None else int(eos_token_id)
         self.stride = int(stride) if stride is not None else self.seq_len
         self.dtype = np.dtype(dtype)
         self._tokens = None            # opened lazily: a memmap must not be pickled into DataLoader workers
@@ -89,12 +97,26 @@ class TokenFileDataset(Dataset):
             raise IndexError(i)
         start = i * self.stride
         chunk = np.asarray(self._open()[start:start + self.seq_len]).astype(np.int64)
-        return {"input_ids": torch.from_numpy(chunk)}
+        item = {"input_ids": torch.from_numpy(chunk)}
+        if self.eos_token_id is not None:
+            item["position_ids"] = torch.from_numpy(_packed_positions(chunk, self.eos_token_id))
+        return item
 
     def __getstate__(self):
         state = dict(self.__dict__)
         state["_tokens"] = None
         return state
+
+
+def _packed_positions(tokens, eos_token_id: int):
+    """int64 positions of a window of concatenated documents: ``arange`` restarted after every ``eos_token_id``."""
+    import numpy as np
+
+    n = tokens.shape[0]
+    idx = np.arange(n, dtype=np.int64)
+    start = np.zeros(n, dtype=np.int64)
+    start[1:] = np.where(tokens[:-1] == eos_token_id, idx[1:], 0)
+    return idx - np.maximum.accumulate(start)
 
 
 def write_token_file(path: str, tokens: Union[torch.Tensor, Iterable[int]], dtype: str = "uint16") -> None:
