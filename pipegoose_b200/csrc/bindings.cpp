@@ -337,6 +337,42 @@ void attention_bwd(const torch::Tensor& qkv, const torch::Tensor& slopes, const 
                                dq_acc.data_ptr<float>(), delta.data_ptr<float>(), (int)B, (int)S, (int)H, (int)D, (float)softmax_scale, seg, cur_stream()) == 0, "attention_bwd failed");
 }
 
+// One decoding step (decode_sm90.cu): writes the new k / v of qkv [B, H*3*D] at column pos of k_cache / v_cache
+// [B, H, capacity, D] and returns attention over keys lead[b] .. pos in out [B, H*D].  ticket: int32, at least B*H
+// entries, all zero (the kernel leaves them zero).
+void decode_attention(const torch::Tensor& qkv, torch::Tensor k_cache, torch::Tensor v_cache, const torch::Tensor& slopes,
+                      int64_t pos, const c10::optional<torch::Tensor>& lead, torch::Tensor out, torch::Tensor ticket,
+                      double softmax_scale) {
+  PG_CUDA(qkv); PG_BF16(qkv); PG_CUDA(k_cache); PG_BF16(k_cache); PG_CUDA(v_cache); PG_BF16(v_cache);
+  PG_CUDA(out); PG_BF16(out); PG_CUDA(slopes); PG_F32(slopes); PG_CUDA(ticket);
+  TORCH_CHECK(ticket.scalar_type() == torch::kInt32, "ticket must be int32");
+  TORCH_CHECK(k_cache.dim() == 4 && v_cache.sizes() == k_cache.sizes(), "k_cache / v_cache must be [B, H, capacity, D]");
+  const int64_t B = k_cache.size(0), H = k_cache.size(1), cap = k_cache.size(2), D = k_cache.size(3);
+  TORCH_CHECK(D == 64 || D == 80 || D == 128, "decode_attention: head size ", D, " has no kernel (64, 80, 128)");
+  TORCH_CHECK(qkv.numel() == B * H * 3 * D && out.numel() == B * H * D && slopes.numel() == H, "decode_attention: shape mismatch");
+  TORCH_CHECK(ticket.numel() >= B * H, "ticket must hold at least B*H = ", B * H, " entries");
+  TORCH_CHECK(0 <= pos && pos < cap, "decode_attention: pos ", pos, " outside the cache capacity ", cap);
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&qkv, &k_cache, &v_cache, &out, &slopes, &ticket})
+    TORCH_CHECK(t->device() == qkv.device(), "decode_attention: tensors on different devices");
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&qkv, &k_cache, &v_cache})
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, "decode_attention: qkv and caches must be 16B aligned");
+  const int* lp = nullptr;
+  if (lead.has_value()) {
+    PG_CUDA(*lead);
+    TORCH_CHECK(lead->scalar_type() == torch::kInt32 && lead->numel() == B && lead->device() == qkv.device(),
+                "lead must be int32 [B] on the device of qkv");
+    lp = lead->data_ptr<int>();
+  }
+  c10::cuda::CUDAGuard guard(qkv.device());
+  const int splits = pg_decode_splits((int)B, (int)H, (int)pos + 1);
+  torch::Tensor part;
+  if (splits > 1) part = torch::empty({B * H * splits * (D + 2)}, qkv.options().dtype(torch::kFloat32));
+  TORCH_CHECK(pg_decode_attention(qkv.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), slopes.data_ptr<float>(), lp,
+                                  out.data_ptr(), splits > 1 ? part.data_ptr<float>() : nullptr, ticket.data_ptr<int>(),
+                                  (int)B, (int)H, (int)D, (int)cap, (int)pos, splits, (float)softmax_scale,
+                                  cur_stream()) == 0, "decode_attention failed");
+}
+
 void moe_route(const torch::Tensor& x, const torch::Tensor& wg, const c10::optional<torch::Tensor>& bg,
                const c10::optional<torch::Tensor>& jitter, int64_t top_k, int64_t capacity, torch::Tensor probs,
                torch::Tensor topk_idx, torch::Tensor topk_prob, torch::Tensor pos, torch::Tensor counts,
@@ -510,6 +546,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("attention_bwd", &attention_bwd, py::arg("qkv"), py::arg("slopes"), py::arg("out"), py::arg("lse"), py::arg("dout"),
         py::arg("dqkv"), py::arg("B"), py::arg("S"), py::arg("H"), py::arg("D"), py::arg("softmax_scale") = 0.0,
         py::arg("seg_start") = py::none());
+  m.def("decode_attention", &decode_attention, py::arg("qkv"), py::arg("k_cache"), py::arg("v_cache"), py::arg("slopes"),
+        py::arg("pos"), py::arg("lead"), py::arg("out"), py::arg("ticket"), py::arg("softmax_scale") = 0.0);
   m.def("moe_route", &moe_route);
   m.def("moe_dispatch", &moe_dispatch);
   m.def("symm_alloc", &symm_alloc);

@@ -81,6 +81,17 @@ int pg_attention_bwd(const void* qkv, const float* slopes, const void* out, cons
                      void* dqkv, float* dq_acc, float* delta, int B, int S, int H, int D, float softmax_scale,
                      const int* seg_start, cudaStream_t s);
 
+// ---- decode_sm90.cu
+// One decoding step of B rows at column pos: writes the new k / v of qkv [B, H*3*D] into k_cache / v_cache
+// [B, H, capacity, D], then out [B, H*D] = softmax(q.k * scale + slope * (k - pos)) V over keys lead[b] <= k <= pos
+// (lead: int32 [B] or nullptr).  D in {64, 80, 128}.  splits > 1: part is an fp32 workspace of B*H*splits*(D+2)
+// floats and ticket an int32 [B*H] array that is zero before the call and zero again after it.
+int pg_decode_attention(const void* qkv, void* k_cache, void* v_cache, const float* slopes, const int* lead, void* out,
+                        float* part, int* ticket, int B, int H, int D, int capacity, int pos, int splits,
+                        float softmax_scale, cudaStream_t s);
+// split count for B*H rows whose key ranges are at most `span` keys long
+int pg_decode_splits(int B, int H, int span);
+
 // ---- moe.cu
 int pg_moe_route(const void* x, const void* wg, const void* bg, const float* jitter, int n, int h, int E, int top_k,
                  int capacity, float* probs, int* topk_idx, float* topk_prob, int* pos, int* counts,

@@ -457,7 +457,9 @@ class BloomForCausalLM(nn.Module):
         then counts the tokens of one decoding step, not of the whole sequence — with a limit that binds, cached and
         uncached decoding may drop different tokens).  🤗's left-padded prompts of unequal length (``attention_mask`` with
         leading zeros) are cached too: pad keys are masked per row, ALiBi only sees distances between real tokens.
-        Masks that are not left-padded are refused (the new tokens go behind the last column).  Recomputed through the
+        Masks that are not left-padded are refused (the new tokens go behind the last column).  On CUDA bf16 models whose
+        head size is 64, 80 or 128 the cache is preallocated for ``prompt + max_new_tokens`` positions, the prompt runs
+        through the flash kernel and every new token through the split-KV decode kernel.  Recomputed through the
         training forward for every token instead: models with a fused NVLink MoE layer (kernels built around
         token-sharded full sequences), ``use_cache=False``, and pipelined models (``PipelineParallel``: one forward-only
         schedule per token, the last stage picks the token and broadcasts it to the other stages)."""
@@ -484,7 +486,8 @@ class BloomForCausalLM(nn.Module):
         for step in range(max_new_tokens):
             if cached:
                 last = self._incremental_logits(out if step == 0 else out[:, -1:], cache,
-                                                0 if step == 0 else out.shape[1] - 1, lead)[:, -1, :]
+                                                0 if step == 0 else out.shape[1] - 1, lead,
+                                                capacity=prompt_len + max_new_tokens)[:, -1, :]
             else:
                 S = out.shape[1]
                 pad = 0
@@ -565,13 +568,17 @@ class BloomForCausalLM(nn.Module):
         return nxt
 
     def _incremental_logits(self, ids: torch.Tensor, cache: list, past: int,
-                            lead: Optional[torch.Tensor] = None) -> torch.Tensor:
+                            lead: Optional[torch.Tensor] = None, capacity: Optional[int] = None) -> torch.Tensor:
         """Inference-only forward of ``ids`` (positions ``past .. past+T-1``) against the cached keys / values; plain
         tensor ops on the module's weights (the fused training kernels are built around full sequences).  ``lead[b]``:
         number of pad positions in front of row ``b`` (left-padded batch; None: no pads) — pad keys are masked with a
         large finite negative (a pad QUERY then attends uniformly instead of producing NaNs that ``0 * NaN`` would
         carry into real rows), learned absolute positions count from the first real token.  ALiBi needs no shift:
-        ``slope * key_position`` differs from 🤗's mask-derived bias by a per-row constant, which softmax ignores."""
+        ``slope * key_position`` differs from 🤗's mask-derived bias by a per-row constant, which softmax ignores.
+
+        CUDA bf16 models whose head size has a decode kernel run attention natively instead (:func:`_cached_attention`):
+        the keys / values live in buffers of ``capacity`` positions (default: the prompt length) allocated at the
+        prompt, which goes through the flash kernel; every later call appends one position."""
         import torch.nn.functional as F
 
         t, cfg = self.transformer, self.config
@@ -580,7 +587,10 @@ class BloomForCausalLM(nn.Module):
         D = h // n_head
         tp = self.tp
         if tp is not None:
-            return self._incremental_logits_tp(ids, cache, past, lead)
+            return self._incremental_logits_tp(ids, cache, past, lead, capacity)
+        native = _native_decode(t.h[0].self_attention.query_key_value.weight, D)
+        if native and lead is not None:
+            lead = lead.to(torch.int32)          # the kernels' type, converted once for every layer
         x = F.embedding(ids, t.word_embeddings.weight)
         if getattr(cfg, "position_embedding", "alibi") == "learned":
             x = x + _learned_positions(t.position_embeddings.weight, past, T, lead)
@@ -589,20 +599,24 @@ class BloomForCausalLM(nn.Module):
         for li, block in enumerate(t.h):
             attn = block.self_attention
             ln = F.layer_norm(x, (h,), block.input_layernorm.weight, block.input_layernorm.bias, block.eps)
-            qkv = F.linear(ln, attn.query_key_value.weight, attn.query_key_value.bias).view(B, T, n_head, 3, D)
-            q, k, v = (qkv[:, :, :, i].transpose(1, 2) for i in range(3))               # [B, H, T, D]
-            if cache[li] is not None:
-                k, v = torch.cat([cache[li][0], k], dim=2), torch.cat([cache[li][1], v], dim=2)
-            cache[li] = (k, v)
-            S = k.shape[2]
-            scores = torch.matmul(q.float(), k.float().transpose(-1, -2)) / math.sqrt(D)   # [B, H, T, S]
-            key_pos = torch.arange(S, device=ids.device, dtype=torch.float32)
-            if attn.use_alibi:
-                scores = scores + K.alibi_slopes(n_head, device=ids.device).view(1, n_head, 1, 1) * key_pos
-            query_pos = torch.arange(past, past + T, device=ids.device).view(T, 1)
-            scores = scores.masked_fill(key_pos.view(1, S) > query_pos, float("-inf"))
-            scores = _mask_leading_pads(scores, key_pos, lead)
-            ctx = torch.matmul(scores.softmax(-1).to(v.dtype), v).transpose(1, 2).reshape(B, T, h)
+            qkv = F.linear(ln, attn.query_key_value.weight, attn.query_key_value.bias)
+            if native:
+                ctx = _cached_attention(qkv, attn.alibi_slopes_local(n_head), cache, li, past, lead, capacity, n_head, D)
+            else:
+                qkv = qkv.view(B, T, n_head, 3, D)
+                q, k, v = (qkv[:, :, :, i].transpose(1, 2) for i in range(3))               # [B, H, T, D]
+                if cache[li] is not None:
+                    k, v = torch.cat([cache[li][0], k], dim=2), torch.cat([cache[li][1], v], dim=2)
+                cache[li] = (k, v)
+                S = k.shape[2]
+                scores = torch.matmul(q.float(), k.float().transpose(-1, -2)) / math.sqrt(D)   # [B, H, T, S]
+                key_pos = torch.arange(S, device=ids.device, dtype=torch.float32)
+                if attn.use_alibi:
+                    scores = scores + K.alibi_slopes(n_head, device=ids.device).view(1, n_head, 1, 1) * key_pos
+                query_pos = torch.arange(past, past + T, device=ids.device).view(T, 1)
+                scores = scores.masked_fill(key_pos.view(1, S) > query_pos, float("-inf"))
+                scores = _mask_leading_pads(scores, key_pos, lead)
+                ctx = torch.matmul(scores.softmax(-1).to(v.dtype), v).transpose(1, 2).reshape(B, T, h)
             x = x + F.linear(ctx, attn.dense.weight, attn.dense.bias)
             ln = F.layer_norm(x, (h,), block.post_attention_layernorm.weight, block.post_attention_layernorm.bias, block.eps)
             mlp = block.mlp
@@ -615,7 +629,7 @@ class BloomForCausalLM(nn.Module):
         return F.linear(x, self.lm_head.weight)
 
     def _incremental_logits_tp(self, ids: torch.Tensor, cache: list, past: int,
-                               lead: Optional[torch.Tensor] = None) -> torch.Tensor:
+                               lead: Optional[torch.Tensor] = None, capacity: Optional[int] = None) -> torch.Tensor:
         """:meth:`_incremental_logits` on a tensor-parallel model: activations are replicated ``[B, T, h]`` (decoding is
         latency-bound: no sequence sharding), every rank runs the attention heads / MLP columns / vocabulary rows it owns
         and caches ITS heads' keys and values; row-parallel products and the embedding are summed over the group, the
@@ -628,6 +642,9 @@ class BloomForCausalLM(nn.Module):
         B, T = ids.shape
         h = cfg.hidden_size
         D = h // cfg.n_head
+        native = _native_decode(t.h[0].self_attention.query_key_value.weight, D)
+        if native and lead is not None:
+            lead = lead.to(torch.int32)
 
         def all_reduce(x):
             dist.all_reduce(x, group=group)
@@ -646,19 +663,23 @@ class BloomForCausalLM(nn.Module):
             attn, mlp = block.self_attention, block.mlp
             n_local = attn.query_key_value.weight.shape[0] // (3 * D)
             ln = F.layer_norm(x, (h,), block.input_layernorm.weight, block.input_layernorm.bias, block.eps)
-            qkv = F.linear(ln, attn.query_key_value.weight, attn.query_key_value.bias).view(B, T, n_local, 3, D)
-            q, k, v = (qkv[:, :, :, i].transpose(1, 2) for i in range(3))               # [B, H/world, T, D]
-            if cache[li] is not None:
-                k, v = torch.cat([cache[li][0], k], dim=2), torch.cat([cache[li][1], v], dim=2)
-            cache[li] = (k, v)
-            S = k.shape[2]
-            scores = torch.matmul(q.float(), k.float().transpose(-1, -2)) / math.sqrt(D)
-            key_pos = torch.arange(S, device=ids.device, dtype=torch.float32)
-            scores = scores + attn.alibi_slopes_local(n_local).view(1, n_local, 1, 1) * key_pos
-            query_pos = torch.arange(past, past + T, device=ids.device).view(T, 1)
-            scores = scores.masked_fill(key_pos.view(1, S) > query_pos, float("-inf"))
-            scores = _mask_leading_pads(scores, key_pos, lead)
-            ctx = torch.matmul(scores.softmax(-1).to(v.dtype), v).transpose(1, 2).reshape(B, T, n_local * D)
+            qkv = F.linear(ln, attn.query_key_value.weight, attn.query_key_value.bias)
+            if native:
+                ctx = _cached_attention(qkv, attn.alibi_slopes_local(n_local), cache, li, past, lead, capacity, n_local, D)
+            else:
+                qkv = qkv.view(B, T, n_local, 3, D)
+                q, k, v = (qkv[:, :, :, i].transpose(1, 2) for i in range(3))               # [B, H/world, T, D]
+                if cache[li] is not None:
+                    k, v = torch.cat([cache[li][0], k], dim=2), torch.cat([cache[li][1], v], dim=2)
+                cache[li] = (k, v)
+                S = k.shape[2]
+                scores = torch.matmul(q.float(), k.float().transpose(-1, -2)) / math.sqrt(D)
+                key_pos = torch.arange(S, device=ids.device, dtype=torch.float32)
+                scores = scores + attn.alibi_slopes_local(n_local).view(1, n_local, 1, 1) * key_pos
+                query_pos = torch.arange(past, past + T, device=ids.device).view(T, 1)
+                scores = scores.masked_fill(key_pos.view(1, S) > query_pos, float("-inf"))
+                scores = _mask_leading_pads(scores, key_pos, lead)
+                ctx = torch.matmul(scores.softmax(-1).to(v.dtype), v).transpose(1, 2).reshape(B, T, n_local * D)
             x = x + all_reduce(F.linear(ctx, attn.dense.weight)) + attn.dense.bias      # row-parallel: bias once
             ln = F.layer_norm(x, (h,), block.post_attention_layernorm.weight, block.post_attention_layernorm.bias, block.eps)
             if not isinstance(mlp, BloomMLP):
@@ -700,6 +721,53 @@ class BloomForCausalLM(nn.Module):
     def save_hf_pretrained(self, path: str, **kwargs) -> None:
         """``to_hf().save_pretrained(path)``: a directory 🤗 ``from_pretrained`` reads (config.json + weights)."""
         self.to_hf().save_pretrained(path, **kwargs)
+
+
+def _native_decode(qkv_weight: torch.Tensor, D: int) -> bool:
+    """Does KV-cached decoding run attention on the sm_90a kernels (CUDA bf16 weights, a head size the decode kernel
+    has)?  Otherwise the eager attention of ``_incremental_logits`` runs."""
+    from pipegoose_b200.ops import use_native
+    from pipegoose_b200.ops.attention import DECODE_HEAD_DIMS
+
+    return use_native(qkv_weight) and D in DECODE_HEAD_DIMS
+
+
+def _cached_attention(qkv: torch.Tensor, slopes: torch.Tensor, cache: list, li: int, past: int,
+                      lead: Optional[torch.Tensor], capacity: Optional[int], n_head: int, D: int) -> torch.Tensor:
+    """Native attention of layer ``li`` for ``qkv [B, T, n_head*3*D]`` at positions ``past .. past+T-1``: the prompt
+    (``past == 0``) through the flash kernel, whose document starts express the left pads (a real token of row b sees
+    keys from ``lead[b]`` on, a pad sees the pads in front of it), then copied once into fresh ``[B, n_head, capacity,
+    D]`` buffers; one new position (``T == 1``) through the split-KV decode kernel, which appends to them.
+    ``cache[li]`` is ``(k[:, :, :filled], v[:, :, :filled], k_buffer, v_buffer)``.  Returns ``[B, T, n_head*D]``."""
+    from pipegoose_b200.ops.attention import alibi_attention, alibi_decode_attention
+
+    B, T = qkv.shape[:2]
+    if past == 0 and cache[li] is None:
+        capacity = T if capacity is None else capacity
+        if capacity < T:
+            raise ValueError(f"KV cache capacity {capacity} is smaller than the prompt ({T} positions)")
+        seg = None
+        if lead is not None:
+            s = torch.arange(T, device=qkv.device).view(1, T)
+            first = lead.view(B, 1).to(s.dtype)
+            seg = torch.where(s >= first, first, torch.zeros_like(first)).to(torch.int32)
+        ctx = alibi_attention(qkv.reshape(B * T, -1), slopes, B, T, n_head, D, seg_start=seg)
+        kv = qkv.view(B, T, n_head, 3, D)
+        k_buf = qkv.new_empty(B, n_head, capacity, D)
+        v_buf = qkv.new_empty(B, n_head, capacity, D)
+        k_buf[:, :, :T].copy_(kv[:, :, :, 1].transpose(1, 2))
+        v_buf[:, :, :T].copy_(kv[:, :, :, 2].transpose(1, 2))
+        cache[li] = (k_buf[:, :, :T], v_buf[:, :, :T], k_buf, v_buf)
+        return ctx.view(B, T, n_head * D)
+    if T != 1 or cache[li] is None or cache[li][0].shape[2] != past:
+        raise ValueError(f"the native KV cache takes a prompt at position 0 and then one token per call "
+                         f"(got {T} positions at {past})")
+    k_buf, v_buf = cache[li][2], cache[li][3]
+    if past >= k_buf.shape[2]:
+        raise ValueError(f"KV cache full: position {past} is past its capacity of {k_buf.shape[2]}")
+    ctx = alibi_decode_attention(qkv.view(B, -1), k_buf, v_buf, slopes, past, lead, D)
+    cache[li] = (k_buf[:, :, :past + 1], v_buf[:, :, :past + 1], k_buf, v_buf)
+    return ctx.view(B, 1, n_head * D)
 
 
 def _mask_leading_pads(scores: torch.Tensor, key_pos: torch.Tensor, lead: Optional[torch.Tensor]) -> torch.Tensor:

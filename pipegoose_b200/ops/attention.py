@@ -181,3 +181,70 @@ def alibi_attention(qkv: torch.Tensor, slopes: torch.Tensor, B: int, S: int, n_h
         out = torch.nn.functional.scaled_dot_product_attention(q, k, v, attn_mask=bias)
         return out.permute(0, 2, 1, 3).reshape(B * S, n_head * D)
     return alibi_attention_reference(qkv, slopes, B, S, n_head, D, seg_start=seg_start)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# One decoding step against a preallocated KV cache.
+#
+# ``qkv_new`` is the step's QKV projection ``[B, n_head*3*D]`` (one token per row, same per-head layout as above),
+# ``k_cache`` / ``v_cache`` are ``[B, n_head, capacity, D]``.  Every row appends its token at the same column ``pos``
+# (a left-padded batch grows behind its last column).  The new k / v are written into ``cache[:, :, pos]``; row b's query
+# then attends to keys ``lead[b] <= k <= pos`` with ``q.k * scale + slope[head] * (k - pos)``, which is the ALiBi
+# score ``slope * k`` of the training path shifted by a per-row constant the softmax ignores.
+# ---------------------------------------------------------------------------------------------------------------------
+
+DECODE_HEAD_DIMS = (64, 80, 128)
+_decode_tickets = {}
+
+
+def alibi_decode_attention_reference(qkv_new: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor,
+                                     slopes: torch.Tensor, pos: int, lead, D: int,
+                                     softmax_scale: float = 0.0) -> torch.Tensor:
+    """fp32 PyTorch form of :func:`alibi_decode_attention` (CPU path, test oracle).  ``lead``: int ``[B]`` leading pads
+    per row or None; ``lead[b] > pos`` counts as ``pos``."""
+    B, n_head, capacity = k_cache.shape[:3]
+    if not 0 <= pos < capacity:
+        raise ValueError(f"decode position {pos} is outside the cache capacity {capacity}")
+    x = qkv_new.view(B, n_head, 3, D)
+    k_cache[:, :, pos] = x[:, :, 1]
+    v_cache[:, :, pos] = x[:, :, 2]
+    q = x[:, :, 0].float()
+    k, v = k_cache[:, :, :pos + 1].float(), v_cache[:, :, :pos + 1].float()
+    scale = softmax_scale if softmax_scale > 0 else 1.0 / math.sqrt(D)
+    scores = torch.einsum("bhd,bhkd->bhk", q, k) * scale
+    key_pos = torch.arange(pos + 1, device=qkv_new.device)
+    scores = scores + slopes.float().view(1, n_head, 1) * (key_pos - pos).float()
+    if lead is not None:
+        hidden = key_pos.view(1, 1, -1) < lead.to(key_pos.device).clamp(max=pos).view(-1, 1, 1)
+        scores = scores.masked_fill(hidden, float("-inf"))
+    out = torch.einsum("bhk,bhkd->bhd", scores.softmax(-1), v)
+    return out.reshape(B, n_head * D).to(qkv_new.dtype)
+
+
+def _decode_ticket(n: int, device) -> torch.Tensor:
+    """The kernel's per-(row, head) arrival counters: zero between calls (the last CTA of each pair resets its own), so
+    one zeroed array per device serves every call on that device's stream."""
+    t = _decode_tickets.get(device)
+    if t is None or t.numel() < n:
+        t = torch.zeros(max(n, 4096), dtype=torch.int32, device=device)
+        _decode_tickets[device] = t
+    return t
+
+
+def alibi_decode_attention(qkv_new: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, slopes: torch.Tensor,
+                           pos: int, lead, D: int, softmax_scale: float = 0.0) -> torch.Tensor:
+    """One decoding step (section comment above): returns ``[B, n_head*D]`` and writes the new keys and values into
+    the caches.  CUDA bf16 inputs run the split-KV kernel (``csrc/decode_sm90.cu``, D in 64 / 80 / 128); ``lead`` is
+    then an int tensor ``[B]`` on the same device, or None."""
+    if not use_native(qkv_new):
+        return alibi_decode_attention_reference(qkv_new, k_cache, v_cache, slopes, pos, lead, D, softmax_scale)
+    if D not in DECODE_HEAD_DIMS:
+        raise ValueError(f"the decode-attention kernel has no head size {D} (supported: {DECODE_HEAD_DIMS})")
+    B, n_head, capacity = k_cache.shape[:3]
+    if not 0 <= pos < capacity:
+        raise ValueError(f"decode position {pos} is outside the cache capacity {capacity}")
+    out = torch.empty(B, n_head * D, dtype=qkv_new.dtype, device=qkv_new.device)
+    lead32 = None if lead is None else lead.to(torch.int32).contiguous()
+    native().decode_attention(qkv_new.contiguous(), k_cache, v_cache, slopes.float().contiguous(), int(pos), lead32,
+                              out, _decode_ticket(B * n_head, qkv_new.device), softmax_scale)
+    return out
