@@ -392,6 +392,9 @@ void moe_dispatch(const torch::Tensor& x, const torch::Tensor& topk_idx, const t
   PG_CUDA(x); PG_BF16(x);
   c10::cuda::CUDAGuard guard(x.device());
   const int T = (int)peer_buf.size();
+  TORCH_CHECK(T >= 1 && T <= PG_MAX_PEERS, "moe_dispatch: 1..", PG_MAX_PEERS, " peer buffers, got ", T);
+  TORCH_CHECK(peer_row_ret.size() == peer_buf.size() && peer_row_scale.size() == peer_buf.size() &&
+                  peer_arrive.size() == peer_buf.size(), "moe_dispatch: the four peer lists must have the same length");
   void* bufs[PG_MAX_PEERS]; int* rets[PG_MAX_PEERS]; float* scs[PG_MAX_PEERS]; uint32_t* arr[PG_MAX_PEERS];
   for (int i = 0; i < T; ++i) { bufs[i] = reinterpret_cast<void*>(peer_buf[i]); rets[i] = reinterpret_cast<int*>(peer_row_ret[i]);
     scs[i] = reinterpret_cast<float*>(peer_row_scale[i]); arr[i] = reinterpret_cast<uint32_t*>(peer_arrive[i]); }

@@ -88,6 +88,17 @@ __global__ void __launch_bounds__(256) moe_route_kernel(
         probs[static_cast<size_t>(t) * E + e] = p[e];
         atomicAdd(&prob_sum[e], p[e]);
       }
+      // A token whose probabilities are not finite (a NaN or +-inf input, weight or logit makes all of them NaN) is
+      // dropped for every k: expert 0, weight 0, no slot, not counted.  Its NaN still reaches probs / lse / prob_sum /
+      // zsum, and so the losses, as on the eager path.
+      if (!isfinite(lse)) {
+        for (int k = 0; k < top_k; ++k) {
+          topk_idx[t * top_k + k] = 0;
+          topk_prob[t * top_k + k] = 0.f;
+          pos[t * top_k + k] = -1;
+        }
+        continue;
+      }
       int chosen[kMaxTopK] = {-1, -1};
       for (int k = 0; k < top_k; ++k) {
         int best = -1;
@@ -183,7 +194,8 @@ extern "C" int pg_moe_route(const void* x, const void* wg, const void* bg, const
                             int top_k, int capacity, float* probs, int* topk_idx, float* topk_prob, int* pos,
                             int* counts, float* prob_sum, float* zsum, float* lse_out, cudaStream_t s) {
   if (n == 0) return 0;
-  if (E > kMaxExperts || top_k > kMaxTopK || h % 8 != 0) return -1;
+  // top_k distinct experts must exist: with top_k > E the last picks would find no expert
+  if (E < 1 || E > kMaxExperts || top_k < 1 || top_k > kMaxTopK || top_k > E || h % 8 != 0) return -1;
   const size_t smem = static_cast<size_t>(E) * h * 2;
   if (smem > 200 * 1024) return -1;
   static bool set = false;
