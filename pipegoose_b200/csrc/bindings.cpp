@@ -373,6 +373,63 @@ void decode_attention(const torch::Tensor& qkv, torch::Tensor k_cache, torch::Te
                                   cur_stream()) == 0, "decode_attention failed");
 }
 
+void check_pools(const torch::Tensor& qkv, const torch::Tensor& k_pool, const torch::Tensor& v_pool, const char* op) {
+  PG_CUDA(qkv); PG_BF16(qkv); PG_CUDA(k_pool); PG_BF16(k_pool); PG_CUDA(v_pool); PG_BF16(v_pool);
+  TORCH_CHECK(k_pool.dim() == 4 && v_pool.sizes() == k_pool.sizes(), op, ": k_pool / v_pool must be [num_pages, H, 64, D]");
+  TORCH_CHECK(k_pool.size(2) == 64, op, ": the pools' page dimension must be 64, got ", k_pool.size(2));
+  const int64_t D = k_pool.size(3);
+  TORCH_CHECK(D == 64 || D == 80 || D == 128, op, ": head size ", D, " has no kernel (64, 80, 128)");
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&k_pool, &v_pool})
+    TORCH_CHECK(t->device() == qkv.device(), op, ": tensors on different devices");
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&qkv, &k_pool, &v_pool})
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, op, ": qkv and pools must be 16B aligned");
+}
+
+// One decoding step over paged pools (decode_sm90.cu, PAGED): row b writes its new k / v of qkv [B, H*3*D] at
+// position pos[b] (the slot of page table[b, pos[b] / 64]) and attends to keys 0 .. pos[b]; out [B, H*D].  table
+// (int32 [B, max_pages]) and pos (int32 [B]) stay on the device: the caller guarantees pos[b] <= max_pos, that
+// table[b, 0 .. pos[b] / 64] are pages of the pool and that no two rows share a page.  ticket as for decode_attention.
+void paged_decode_attention(const torch::Tensor& qkv, torch::Tensor k_pool, torch::Tensor v_pool,
+                            const torch::Tensor& table, const torch::Tensor& pos, int64_t max_pos,
+                            const torch::Tensor& slopes, torch::Tensor out, torch::Tensor ticket, double softmax_scale) {
+  check_pools(qkv, k_pool, v_pool, "paged_decode_attention");
+  PG_CUDA(out); PG_BF16(out); PG_CUDA(slopes); PG_F32(slopes); PG_CUDA(ticket); PG_CUDA(table); PG_CUDA(pos);
+  TORCH_CHECK(ticket.scalar_type() == torch::kInt32 && table.scalar_type() == torch::kInt32 &&
+              pos.scalar_type() == torch::kInt32, "paged_decode_attention: ticket, table and pos must be int32");
+  TORCH_CHECK(table.dim() == 2 && table.size(1) >= 1, "paged_decode_attention: table must be [B, max_pages]");
+  const int64_t B = table.size(0), H = k_pool.size(1), D = k_pool.size(3), max_pages = table.size(1);
+  TORCH_CHECK(pos.numel() == B && qkv.numel() == B * H * 3 * D && out.numel() == B * H * D && slopes.numel() == H,
+              "paged_decode_attention: shape mismatch");
+  TORCH_CHECK(ticket.numel() >= B * H, "ticket must hold at least B*H = ", B * H, " entries");
+  TORCH_CHECK(0 <= max_pos && max_pos < max_pages * 64, "paged_decode_attention: max_pos ", max_pos,
+              " outside the ", max_pages, " pages of a table row");
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&out, &slopes, &ticket, &table, &pos})
+    TORCH_CHECK(t->device() == qkv.device(), "paged_decode_attention: tensors on different devices");
+  if (B == 0) return;
+  c10::cuda::CUDAGuard guard(qkv.device());
+  const int splits = pg_decode_splits((int)B, (int)H, (int)max_pos + 1);
+  torch::Tensor part;
+  if (splits > 1) part = torch::empty({B * H * splits * (D + 2)}, qkv.options().dtype(torch::kFloat32));
+  TORCH_CHECK(pg_paged_decode_attention(qkv.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(), table.data_ptr<int>(),
+                                        pos.data_ptr<int>(), slopes.data_ptr<float>(), out.data_ptr(),
+                                        splits > 1 ? part.data_ptr<float>() : nullptr, ticket.data_ptr<int>(), (int)B,
+                                        (int)H, (int)D, (int)max_pages, (int)max_pos, splits, (float)softmax_scale,
+                                        cur_stream()) == 0, "paged_decode_attention failed");
+}
+
+// Prefill cache write: the k / v of every token n of qkv [N, H*3*D] into pool slot slot[n] (page * 64 + offset).  The
+// caller guarantees every slot lies in the pool.
+void paged_kv_write(const torch::Tensor& qkv, const torch::Tensor& slot, torch::Tensor k_pool, torch::Tensor v_pool) {
+  check_pools(qkv, k_pool, v_pool, "paged_kv_write");
+  PG_CUDA(slot);
+  TORCH_CHECK(slot.scalar_type() == torch::kInt32 && slot.device() == qkv.device(), "paged_kv_write: slot must be int32 on the device of qkv");
+  const int64_t N = slot.numel(), H = k_pool.size(1), D = k_pool.size(3);
+  TORCH_CHECK(qkv.numel() == N * H * 3 * D, "paged_kv_write: qkv must be [N, H*3*D] for the N = ", N, " slots");
+  c10::cuda::CUDAGuard guard(qkv.device());
+  TORCH_CHECK(pg_paged_kv_write(qkv.data_ptr(), slot.data_ptr<int>(), k_pool.data_ptr(), v_pool.data_ptr(), (int)N,
+                                (int)H, (int)D, cur_stream()) == 0, "paged_kv_write failed");
+}
+
 void moe_route(const torch::Tensor& x, const torch::Tensor& wg, const c10::optional<torch::Tensor>& bg,
                const c10::optional<torch::Tensor>& jitter, int64_t top_k, int64_t capacity, torch::Tensor probs,
                torch::Tensor topk_idx, torch::Tensor topk_prob, torch::Tensor pos, torch::Tensor counts,
@@ -551,6 +608,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("seg_start") = py::none());
   m.def("decode_attention", &decode_attention, py::arg("qkv"), py::arg("k_cache"), py::arg("v_cache"), py::arg("slopes"),
         py::arg("pos"), py::arg("lead"), py::arg("out"), py::arg("ticket"), py::arg("softmax_scale") = 0.0);
+  m.def("paged_decode_attention", &paged_decode_attention, py::arg("qkv"), py::arg("k_pool"), py::arg("v_pool"),
+        py::arg("table"), py::arg("pos"), py::arg("max_pos"), py::arg("slopes"), py::arg("out"), py::arg("ticket"),
+        py::arg("softmax_scale") = 0.0);
+  m.def("paged_kv_write", &paged_kv_write, py::arg("qkv"), py::arg("slot"), py::arg("k_pool"), py::arg("v_pool"));
   m.def("moe_route", &moe_route);
   m.def("moe_dispatch", &moe_dispatch);
   m.def("symm_alloc", &symm_alloc);

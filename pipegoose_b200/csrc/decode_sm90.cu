@@ -19,6 +19,16 @@
 // The key at `pos` is read from the qkv row, not from the cache, by the one lane group that handles it; that group
 // also stores it into the cache.  No other thread touches cache[:, :, pos], so the write never races a read and the
 // cache can be read through the non-coherent path.
+//
+// Paged form (PAGED = true, continuous batching): the caches are page pools k_pool / v_pool [num_pages, H, 64, D] and
+// every row has its own position pos[b] (int32 [B] on the device).  Row b's position p lives in page
+// table[b, p / 64] (int32 [B, max_pages]) at slot p % 64.  Row b writes its new k / v into the slot of pos[b] and
+// attends to keys 0 <= k <= pos[b]; there is no lead.  The grid is sized for the longest row (`pos` holds the host's
+// bound on max(pos[b])); each row cuts its own range into `splits` chunks, so the bound only shapes the grid.  Rows
+// own disjoint pages, so the write of pos[b]'s slot races no read either.
+//
+// paged_kv_write_kernel stores the k / v of a packed prefill into the pools: token n's heads go to slot[n]
+// (page * 64 + offset), 16 bytes per thread.
 #include "launch.h"
 #include "pdl_launch.cuh"
 #include "ptx.cuh"
@@ -33,6 +43,8 @@ constexpr int kDecUnroll = 4;        // keys of K and V in flight per lane group
 constexpr int kDecMinChunk = 64;     // fewest keys a split is given
 constexpr int kDecTargetCtas = 132 * 4;
 constexpr float kDecLog2e = 1.4426950408889634f;
+constexpr int kPageShift = 6;        // 64 positions per page of the paged pools
+constexpr int kPageSize = 1 << kPageShift;
 
 struct DecodeArgs {
   const __nv_bfloat16* qkv;
@@ -45,6 +57,10 @@ struct DecodeArgs {
   int* ticket;   // [B*H], zero between calls
   int H, capacity, pos, splits;
   float scale_log2;
+  // paged form only (k_cache / v_cache are then the pools, capacity and lead unused)
+  const int* table;     // [B, max_pages] page ids
+  const int* row_pos;   // [B] each row's new-token position
+  int max_pages;
 };
 
 PG_DEVICE void bf16x8_to_f32(const uint4& r, float* f) {
@@ -57,7 +73,7 @@ PG_DEVICE void bf16x8_to_f32(const uint4& r, float* f) {
   }
 }
 
-template <int D>
+template <int D, bool PAGED>
 __global__ void __launch_bounds__(kDecThreads) decode_attention_kernel(const DecodeArgs a) {
   constexpr int VEC = D / 8;                  // lanes holding a key's dims (8 bf16 = 16 B each)
   constexpr int LPK = VEC <= 8 ? 8 : 16;      // lanes per key: VEC rounded up to a power of two (shuffle reduction)
@@ -71,21 +87,30 @@ __global__ void __launch_bounds__(kDecThreads) decode_attention_kernel(const Dec
   pdl_launch_dependents();
   pdl_wait();
   const int split = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-  const int H = a.H, pos = a.pos;
+  const int H = a.H;
+  const int pos = PAGED ? __ldg(a.row_pos + b) : a.pos;
   const int lane = threadIdx.x & 31;
   const int sub = lane % LPK;
   const int grp = (threadIdx.x >> 5) * KPW + lane / LPK;
   const bool active = sub < VEC;
 
-  const int lo = a.lead != nullptr ? min(max(a.lead[b], 0), pos) : 0;
+  const int lo = !PAGED && a.lead != nullptr ? min(max(a.lead[b], 0), pos) : 0;
   const int chunk = (pos - lo + a.splits) / a.splits;   // ceil((pos - lo + 1) / splits)
   const int k0 = lo + split * chunk;
   const int k1 = min(k0 + chunk, pos + 1);
 
   const size_t bh = static_cast<size_t>(b) * H + h;
   const __nv_bfloat16* row = a.qkv + (static_cast<size_t>(b) * H + h) * 3 * D;
-  const uint4* kc = reinterpret_cast<const uint4*>(a.k_cache + bh * a.capacity * D);
-  const uint4* vc = reinterpret_cast<const uint4*>(a.v_cache + bh * a.capacity * D);
+  const uint4* kc = reinterpret_cast<const uint4*>(PAGED ? a.k_cache : a.k_cache + bh * a.capacity * D);
+  const uint4* vc = reinterpret_cast<const uint4*>(PAGED ? a.v_cache : a.v_cache + bh * a.capacity * D);
+  const int* tab = PAGED ? a.table + static_cast<size_t>(b) * a.max_pages : nullptr;
+  // uint4 offset of key k from kc / vc
+  auto key_at = [&](int k) -> size_t {
+    if constexpr (PAGED)
+      return ((static_cast<size_t>(__ldg(tab + (k >> kPageShift))) * H + h) * kPageSize + (k & (kPageSize - 1))) * VEC;
+    else
+      return static_cast<size_t>(k) * VEC;
+  };
   const uint4* k_new = reinterpret_cast<const uint4*>(row + D);
   const uint4* v_new = reinterpret_cast<const uint4*>(row + 2 * D);
 
@@ -114,11 +139,17 @@ __global__ void __launch_bounds__(kDecThreads) decode_attention_kernel(const Dec
         if (k == pos) {
           kr[u] = k_new[sub];
           vr[u] = v_new[sub];
-          reinterpret_cast<uint4*>(a.k_cache + (bh * a.capacity + pos) * D)[sub] = kr[u];
-          reinterpret_cast<uint4*>(a.v_cache + (bh * a.capacity + pos) * D)[sub] = vr[u];
+          if constexpr (PAGED) {
+            reinterpret_cast<uint4*>(a.k_cache)[key_at(pos) + sub] = kr[u];
+            reinterpret_cast<uint4*>(a.v_cache)[key_at(pos) + sub] = vr[u];
+          } else {
+            reinterpret_cast<uint4*>(a.k_cache + (bh * a.capacity + pos) * D)[sub] = kr[u];
+            reinterpret_cast<uint4*>(a.v_cache + (bh * a.capacity + pos) * D)[sub] = vr[u];
+          }
         } else {
-          kr[u] = __ldg(kc + static_cast<size_t>(k) * VEC + sub);
-          vr[u] = __ldg(vc + static_cast<size_t>(k) * VEC + sub);
+          const size_t at = key_at(k);
+          kr[u] = __ldg(kc + at + sub);
+          vr[u] = __ldg(vc + at + sub);
         }
       }
     }
@@ -220,12 +251,41 @@ __global__ void __launch_bounds__(kDecThreads) decode_attention_kernel(const Dec
     }                                                                               \
   } while (0)
 
-template <int D>
+template <int D, bool PAGED>
 static int launch_decode(const DecodeArgs& a, int B, cudaStream_t s) {
-  if (launch_pdl(decode_attention_kernel<D>, dim3(a.splits, a.H, B), dim3(kDecThreads), 0, s, a) != cudaSuccess)
+  if (launch_pdl(decode_attention_kernel<D, PAGED>, dim3(a.splits, a.H, B), dim3(kDecThreads), 0, s, a) != cudaSuccess)
     return -1;
   PG_CHECK_LAUNCH("decode_attention");
   return 0;
+}
+
+template <bool PAGED>
+static int launch_decode_d(const DecodeArgs& a, int B, int D, cudaStream_t s) {
+  switch (D) {
+    case 64: return launch_decode<64, PAGED>(a, B, s);
+    case 80: return launch_decode<80, PAGED>(a, B, s);
+    case 128: return launch_decode<128, PAGED>(a, B, s);
+    default: return -1;
+  }
+}
+
+__global__ void __launch_bounds__(256) paged_kv_write_kernel(const uint4* __restrict__ qkv, const int* __restrict__ slot,
+                                                             uint4* __restrict__ k_pool, uint4* __restrict__ v_pool,
+                                                             int N, int H, int vec) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;   // (n, h, k|v, 16-byte column)
+  if (i >= static_cast<long long>(N) * H * 2 * vec) return;
+  const int c = static_cast<int>(i % vec);
+  long long r = i / vec;
+  const int kv = static_cast<int>(r & 1);
+  r >>= 1;
+  const int h = static_cast<int>(r % H);
+  const long long n = r / H;
+  const int s = __ldg(slot + n);
+  const uint4 x = __ldg(qkv + ((n * H + h) * 3 + 1 + kv) * vec + c);
+  const size_t dst = ((static_cast<size_t>(s >> kPageShift) * H + h) * kPageSize + (s & (kPageSize - 1))) * vec + c;
+  (kv ? v_pool : k_pool)[dst] = x;
 }
 
 }  // namespace pg
@@ -258,10 +318,45 @@ extern "C" int pg_decode_attention(const void* qkv, void* k_cache, void* v_cache
   a.pos = pos;
   a.splits = splits;
   a.scale_log2 = kDecLog2e * (softmax_scale > 0.f ? softmax_scale : 1.0f / sqrtf(static_cast<float>(D)));
-  switch (D) {
-    case 64: return launch_decode<64>(a, B, s);
-    case 80: return launch_decode<80>(a, B, s);
-    case 128: return launch_decode<128>(a, B, s);
-    default: return -1;
-  }
+  a.table = nullptr;
+  a.row_pos = nullptr;
+  a.max_pages = 0;
+  return launch_decode_d<false>(a, B, D, s);
+}
+
+extern "C" int pg_paged_decode_attention(const void* qkv, void* k_pool, void* v_pool, const int* table, const int* pos,
+                                         const float* slopes, void* out, float* part, int* ticket, int B, int H, int D,
+                                         int max_pages, int max_pos, int splits, float softmax_scale, cudaStream_t s) {
+  if (max_pos < 0 || max_pages < 1 || splits < 1 || (splits > 1 && (part == nullptr || ticket == nullptr))) return -1;
+  DecodeArgs a;
+  a.qkv = static_cast<const __nv_bfloat16*>(qkv);
+  a.k_cache = static_cast<__nv_bfloat16*>(k_pool);
+  a.v_cache = static_cast<__nv_bfloat16*>(v_pool);
+  a.slopes = slopes;
+  a.lead = nullptr;
+  a.out = static_cast<__nv_bfloat16*>(out);
+  a.part = part;
+  a.ticket = ticket;
+  a.H = H;
+  a.capacity = 0;
+  a.pos = max_pos;
+  a.splits = splits;
+  a.scale_log2 = kDecLog2e * (softmax_scale > 0.f ? softmax_scale : 1.0f / sqrtf(static_cast<float>(D)));
+  a.table = table;
+  a.row_pos = pos;
+  a.max_pages = max_pages;
+  return launch_decode_d<true>(a, B, D, s);
+}
+
+extern "C" int pg_paged_kv_write(const void* qkv, const int* slot, void* k_pool, void* v_pool, int N, int H, int D,
+                                 cudaStream_t s) {
+  if (N < 0 || H < 1 || D % 8 != 0) return -1;
+  if (N == 0) return 0;
+  const long long n = static_cast<long long>(N) * H * 2 * (D / 8);
+  if (launch_pdl(paged_kv_write_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, s,
+                 static_cast<const uint4*>(qkv), slot, static_cast<uint4*>(k_pool), static_cast<uint4*>(v_pool), N, H,
+                 D / 8) != cudaSuccess)
+    return -1;
+  PG_CHECK_LAUNCH("paged_kv_write");
+  return 0;
 }

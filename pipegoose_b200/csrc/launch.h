@@ -91,6 +91,15 @@ int pg_decode_attention(const void* qkv, void* k_cache, void* v_cache, const flo
                         float softmax_scale, cudaStream_t s);
 // split count for B*H rows whose key ranges are at most `span` keys long
 int pg_decode_splits(int B, int H, int span);
+// The paged form: k_pool / v_pool [num_pages, H, 64, D]; row b's position p is slot p % 64 of page
+// table[b * max_pages + p / 64].  Row b writes its new k / v at pos[b] (int32 [B], device) and attends to keys
+// 0 <= k <= pos[b].  max_pos >= every pos[b] sizes the grid (splits from pg_decode_splits(B, H, max_pos + 1)).
+int pg_paged_decode_attention(const void* qkv, void* k_pool, void* v_pool, const int* table, const int* pos,
+                              const float* slopes, void* out, float* part, int* ticket, int B, int H, int D,
+                              int max_pages, int max_pos, int splits, float softmax_scale, cudaStream_t s);
+// Prefill: the k / v of every token n of qkv [N, H*3*D] into pool slot slot[n] (page * 64 + offset), all heads.
+int pg_paged_kv_write(const void* qkv, const int* slot, void* k_pool, void* v_pool, int N, int H, int D,
+                      cudaStream_t s);
 
 // ---- moe.cu
 int pg_moe_route(const void* x, const void* wg, const void* bg, const float* jitter, int n, int h, int E, int top_k,

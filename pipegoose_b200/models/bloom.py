@@ -579,8 +579,6 @@ class BloomForCausalLM(nn.Module):
         CUDA bf16 models whose head size has a decode kernel run attention natively instead (:func:`_cached_attention`):
         the keys / values live in buffers of ``capacity`` positions (default: the prompt length) allocated at the
         prompt, which goes through the flash kernel; every later call appends one position."""
-        import torch.nn.functional as F
-
         t, cfg = self.transformer, self.config
         B, T = ids.shape
         h, n_head = cfg.hidden_size, cfg.n_head
@@ -591,33 +589,54 @@ class BloomForCausalLM(nn.Module):
         native = _native_decode(t.h[0].self_attention.query_key_value.weight, D)
         if native and lead is not None:
             lead = lead.to(torch.int32)          # the kernels' type, converted once for every layer
+        positions = _learned_positions(t.position_embeddings.weight, past, T, lead) if _learned(cfg) else None
+
+        def attend(li, attn, qkv):
+            if native:
+                return _cached_attention(qkv, attn.alibi_slopes_local(n_head), cache, li, past, lead, capacity, n_head, D)
+            qkv = qkv.view(B, T, n_head, 3, D)
+            q, k, v = (qkv[:, :, :, i].transpose(1, 2) for i in range(3))               # [B, H, T, D]
+            if cache[li] is not None:
+                k, v = torch.cat([cache[li][0], k], dim=2), torch.cat([cache[li][1], v], dim=2)
+            cache[li] = (k, v)
+            S = k.shape[2]
+            scores = torch.matmul(q.float(), k.float().transpose(-1, -2)) / math.sqrt(D)   # [B, H, T, S]
+            key_pos = torch.arange(S, device=ids.device, dtype=torch.float32)
+            if attn.use_alibi:
+                scores = scores + K.alibi_slopes(n_head, device=ids.device).view(1, n_head, 1, 1) * key_pos
+            query_pos = torch.arange(past, past + T, device=ids.device).view(T, 1)
+            scores = scores.masked_fill(key_pos.view(1, S) > query_pos, float("-inf"))
+            scores = _mask_leading_pads(scores, key_pos, lead)
+            return torch.matmul(scores.softmax(-1).to(v.dtype), v).transpose(1, 2).reshape(B, T, h)
+
+        x = self._inference_layers(self._inference_embed(ids, positions), attend)
+        return self._inference_head(x[:, -1:])
+
+    def _inference_embed(self, ids: torch.Tensor, positions: Optional[torch.Tensor]) -> torch.Tensor:
+        """Token embeddings of the inference-only forwards: plus ``positions`` (rows of the learned position table) on
+        GPT-2-style models, the embedding LayerNorm on Bloom."""
+        import torch.nn.functional as F
+
+        t, cfg = self.transformer, self.config
         x = F.embedding(ids, t.word_embeddings.weight)
-        if getattr(cfg, "position_embedding", "alibi") == "learned":
-            x = x + _learned_positions(t.position_embeddings.weight, past, T, lead)
-        else:
-            x = F.layer_norm(x, (h,), t.word_embeddings_layernorm.weight, t.word_embeddings_layernorm.bias, cfg.layer_norm_epsilon)
-        for li, block in enumerate(t.h):
+        if _learned(cfg):
+            return x + positions
+        return F.layer_norm(x, (cfg.hidden_size,), t.word_embeddings_layernorm.weight, t.word_embeddings_layernorm.bias,
+                            cfg.layer_norm_epsilon)
+
+    def _inference_layers(self, x: torch.Tensor, attend) -> torch.Tensor:
+        """Every block of an inference-only forward on ``x [B, T, h]``: plain tensor ops on the module's weights (the
+        fused training kernels are built around full sequences).  ``attend(li, attn, qkv)`` is the attention of layer
+        ``li`` (``attn``: its ``BloomAttention``), from ``qkv [B, T, n_head*3*D]`` to ``[B, T, n_head*D]``; it is the only
+        step the KV-cached and the paged forwards do differently."""
+        import torch.nn.functional as F
+
+        h = self.config.hidden_size
+        for li, block in enumerate(self.transformer.h):
             attn = block.self_attention
             ln = F.layer_norm(x, (h,), block.input_layernorm.weight, block.input_layernorm.bias, block.eps)
             qkv = F.linear(ln, attn.query_key_value.weight, attn.query_key_value.bias)
-            if native:
-                ctx = _cached_attention(qkv, attn.alibi_slopes_local(n_head), cache, li, past, lead, capacity, n_head, D)
-            else:
-                qkv = qkv.view(B, T, n_head, 3, D)
-                q, k, v = (qkv[:, :, :, i].transpose(1, 2) for i in range(3))               # [B, H, T, D]
-                if cache[li] is not None:
-                    k, v = torch.cat([cache[li][0], k], dim=2), torch.cat([cache[li][1], v], dim=2)
-                cache[li] = (k, v)
-                S = k.shape[2]
-                scores = torch.matmul(q.float(), k.float().transpose(-1, -2)) / math.sqrt(D)   # [B, H, T, S]
-                key_pos = torch.arange(S, device=ids.device, dtype=torch.float32)
-                if attn.use_alibi:
-                    scores = scores + K.alibi_slopes(n_head, device=ids.device).view(1, n_head, 1, 1) * key_pos
-                query_pos = torch.arange(past, past + T, device=ids.device).view(T, 1)
-                scores = scores.masked_fill(key_pos.view(1, S) > query_pos, float("-inf"))
-                scores = _mask_leading_pads(scores, key_pos, lead)
-                ctx = torch.matmul(scores.softmax(-1).to(v.dtype), v).transpose(1, 2).reshape(B, T, h)
-            x = x + F.linear(ctx, attn.dense.weight, attn.dense.bias)
+            x = x + F.linear(attend(li, attn, qkv), attn.dense.weight, attn.dense.bias)
             ln = F.layer_norm(x, (h,), block.post_attention_layernorm.weight, block.post_attention_layernorm.bias, block.eps)
             mlp = block.mlp
             if not isinstance(mlp, BloomMLP):
@@ -625,8 +644,54 @@ class BloomForCausalLM(nn.Module):
                 continue
             x = x + F.linear(K.gelu_tanh(F.linear(ln, mlp.dense_h_to_4h.weight, mlp.dense_h_to_4h.bias)),
                              mlp.dense_4h_to_h.weight, mlp.dense_4h_to_h.bias)
-        x = F.layer_norm(x[:, -1:], (h,), t.ln_f.weight, t.ln_f.bias, cfg.layer_norm_epsilon)
+        return x
+
+    def _inference_head(self, x: torch.Tensor) -> torch.Tensor:
+        """Final LayerNorm and lm_head of the inference-only forwards."""
+        import torch.nn.functional as F
+
+        t, cfg = self.transformer, self.config
+        x = F.layer_norm(x, (cfg.hidden_size,), t.ln_f.weight, t.ln_f.bias, cfg.layer_norm_epsilon)
         return F.linear(x, self.lm_head.weight)
+
+    @torch.no_grad()
+    def _paged_logits(self, ids: torch.Tensor, positions: torch.Tensor, k_pools: torch.Tensor, v_pools: torch.Tensor,
+                      seg_start: Optional[torch.Tensor] = None, slot: Optional[torch.Tensor] = None,
+                      last: Optional[torch.Tensor] = None, table: Optional[torch.Tensor] = None,
+                      max_pos: int = 0) -> torch.Tensor:
+        """Inference-only forward of a set of sequences over paged KV pools (``pipegoose_b200.serving``); ``ids`` and
+        ``positions`` (each token's position in its own sequence) are ``[N]``, ``k_pools`` / ``v_pools`` are
+        ``[n_layer, num_pages, n_head, 64, D]``.  Two modes:
+
+        - prefill (``seg_start`` given): the prompts packed into one row, each a document of the flash kernel's
+          ``seg_start`` (int32 ``[N]``); ``slot`` (int32 ``[N]``) is each token's pool slot (``page * 64 + offset``).
+          Returns the logits at the tokens ``last`` (``[n]``, each prompt's last token): ``[n, V]``.
+        - decode: one new token per sequence; ``table`` (int32 ``[N, max_pages]``) holds each sequence's pages,
+          ``positions`` (int32) its new token's position, ``max_pos >= max(positions)``.  Returns ``[N, V]``.
+
+        CUDA bf16 models with head size 64, 80 or 128 run the flash / paged decode kernels; otherwise (CPU, fp32, other
+        head sizes) their PyTorch references run."""
+        from pipegoose_b200.ops import attention as A
+
+        cfg = self.config
+        n_head = cfg.n_head
+        D = cfg.hidden_size // n_head
+        N = ids.shape[0]
+        native = _native_decode(self.transformer.h[0].self_attention.query_key_value.weight, D)
+        write = A.paged_kv_write if native else A.paged_kv_write_reference
+        decode = A.alibi_paged_decode_attention if native else A.alibi_paged_decode_attention_reference
+        pos_emb = self.transformer.position_embeddings.weight[positions.long()] if _learned(cfg) else None
+
+        def attend(li, attn, qkv):
+            qkv = qkv.view(N, n_head * 3 * D)
+            slopes = attn.alibi_slopes_local(n_head)
+            if seg_start is not None:
+                write(qkv, slot, k_pools[li], v_pools[li], D)
+                return A.alibi_attention(qkv, slopes, 1, N, n_head, D, seg_start=seg_start.view(1, N)).view(1, N, -1)
+            return decode(qkv, k_pools[li], v_pools[li], table, positions, max_pos, slopes, D).view(1, N, -1)
+
+        x = self._inference_layers(self._inference_embed(ids.view(1, N), pos_emb), attend)[0]
+        return self._inference_head(x if seg_start is None else x[last.long()])
 
     def _incremental_logits_tp(self, ids: torch.Tensor, cache: list, past: int,
                                lead: Optional[torch.Tensor] = None, capacity: Optional[int] = None) -> torch.Tensor:
@@ -721,6 +786,11 @@ class BloomForCausalLM(nn.Module):
     def save_hf_pretrained(self, path: str, **kwargs) -> None:
         """``to_hf().save_pretrained(path)``: a directory 🤗 ``from_pretrained`` reads (config.json + weights)."""
         self.to_hf().save_pretrained(path, **kwargs)
+
+
+def _learned(cfg) -> bool:
+    """Learned absolute position embeddings (GPT-2) rather than ALiBi?"""
+    return getattr(cfg, "position_embedding", "alibi") == "learned"
 
 
 def _native_decode(qkv_weight: torch.Tensor, D: int) -> bool:

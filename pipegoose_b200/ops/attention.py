@@ -248,3 +248,97 @@ def alibi_decode_attention(qkv_new: torch.Tensor, k_cache: torch.Tensor, v_cache
     native().decode_attention(qkv_new.contiguous(), k_cache, v_cache, slopes.float().contiguous(), int(pos), lead32,
                               out, _decode_ticket(B * n_head, qkv_new.device), softmax_scale)
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Paged KV cache (continuous batching, ``pipegoose_b200.serving``).
+#
+# ``k_pool`` / ``v_pool`` are ``[num_pages, n_head, PAGE_SIZE, D]``.  Row b's position p lives in page
+# ``table[b, p // PAGE_SIZE]`` at slot ``p % PAGE_SIZE`` (``table``: int32 ``[B, max_pages]``).  Every row has its own
+# new-token position ``pos[b]`` (int32 ``[B]``): the step writes its k / v into that slot, and row b's query attends to
+# keys ``0 <= k <= pos[b]`` with ``q.k * scale + slope[head] * (k - pos[b])``.  ``max_pos`` is a host integer
+# ``>= max(pos)``: it sizes the kernel's grid only.  Neither op reads ``table`` or ``pos`` on the host; their caller
+# guarantees ``pos[b] <= max_pos``, that the pages a row uses are pages of the pool, and that no two rows share one.
+# ---------------------------------------------------------------------------------------------------------------------
+
+PAGE_SIZE = 64
+
+
+def _paged_keys(pool: torch.Tensor, table: torch.Tensor, pos: torch.Tensor, n: int):
+    """fp32 ``pool`` rows of positions ``0 .. n-1`` of every table row as ``[B, n_head, n, D]``, zero behind
+    ``pos[b]`` (a table row may hold anything behind its last used page, and unwritten slots anything at all), and
+    the mask of the positions ``<= pos[b]``."""
+    p = torch.arange(n, device=pool.device)
+    valid = p.view(1, n) <= pos.view(-1, 1).to(p.dtype)
+    pages = torch.where(valid, table.long()[:, p // PAGE_SIZE], torch.zeros_like(valid, dtype=torch.long))
+    rows = pool[pages, :, (p % PAGE_SIZE).view(1, n)].float().masked_fill(~valid.view(*valid.shape, 1, 1), 0.0)
+    return rows.transpose(1, 2), valid
+
+
+def _check_max_pos(max_pos: int, table: torch.Tensor) -> None:
+    if not 0 <= max_pos < table.shape[1] * PAGE_SIZE:
+        raise ValueError(f"max_pos {max_pos} is outside the {table.shape[1]} pages of a table row")
+
+
+def alibi_paged_decode_attention_reference(qkv_new: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
+                                           table: torch.Tensor, pos: torch.Tensor, max_pos: int, slopes: torch.Tensor,
+                                           D: int, softmax_scale: float = 0.0) -> torch.Tensor:
+    """fp32 PyTorch form of :func:`alibi_paged_decode_attention` (CPU path, test oracle)."""
+    _check_max_pos(max_pos, table)
+    B, n_head = table.shape[0], k_pool.shape[1]
+    if B == 0:
+        return qkv_new.new_empty(0, n_head * D)
+    x = qkv_new.view(B, n_head, 3, D)
+    pos = pos.to(table.device).long()
+    page = table.long().gather(1, (pos // PAGE_SIZE).view(B, 1)).view(B)
+    k_pool[page, :, pos % PAGE_SIZE] = x[:, :, 1].to(k_pool.dtype)
+    v_pool[page, :, pos % PAGE_SIZE] = x[:, :, 2].to(v_pool.dtype)
+    k, valid = _paged_keys(k_pool, table, pos, max_pos + 1)
+    v, _ = _paged_keys(v_pool, table, pos, max_pos + 1)
+    scale = softmax_scale if softmax_scale > 0 else 1.0 / math.sqrt(D)
+    scores = torch.einsum("bhd,bhkd->bhk", x[:, :, 0].float(), k) * scale
+    key_pos = torch.arange(max_pos + 1, device=k_pool.device)
+    scores = scores + slopes.float().view(1, n_head, 1) * (key_pos.view(1, 1, -1) - pos.view(B, 1, 1)).float()
+    scores = scores.masked_fill(~valid.view(B, 1, -1), float("-inf"))
+    out = torch.einsum("bhk,bhkd->bhd", scores.softmax(-1), v)
+    return out.reshape(B, n_head * D).to(qkv_new.dtype)
+
+
+def alibi_paged_decode_attention(qkv_new: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
+                                 table: torch.Tensor, pos: torch.Tensor, max_pos: int, slopes: torch.Tensor, D: int,
+                                 softmax_scale: float = 0.0) -> torch.Tensor:
+    """One decoding step of ``B`` independent sequences over the paged pools (section comment above): returns
+    ``[B, n_head*D]`` and writes the new keys and values into the pools.  CUDA bf16 inputs run the paged form of the
+    split-KV kernel (``csrc/decode_sm90.cu``, D in 64 / 80 / 128)."""
+    if not use_native(qkv_new):
+        return alibi_paged_decode_attention_reference(qkv_new, k_pool, v_pool, table, pos, max_pos, slopes, D,
+                                                      softmax_scale)
+    if D not in DECODE_HEAD_DIMS:
+        raise ValueError(f"the decode-attention kernel has no head size {D} (supported: {DECODE_HEAD_DIMS})")
+    _check_max_pos(max_pos, table)
+    B, n_head = table.shape[0], k_pool.shape[1]
+    out = torch.empty(B, n_head * D, dtype=qkv_new.dtype, device=qkv_new.device)
+    native().paged_decode_attention(qkv_new.contiguous(), k_pool, v_pool, table.to(torch.int32).contiguous(),
+                                    pos.to(torch.int32).contiguous(), int(max_pos), slopes.float().contiguous(), out,
+                                    _decode_ticket(B * n_head, qkv_new.device), softmax_scale)
+    return out
+
+
+def paged_kv_write_reference(qkv: torch.Tensor, slot: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
+                             D: int) -> None:
+    """PyTorch form of :func:`paged_kv_write`."""
+    n_head = k_pool.shape[1]
+    x = qkv.view(-1, n_head, 3, D)
+    slot = slot.to(k_pool.device).long()
+    k_pool[slot // PAGE_SIZE, :, slot % PAGE_SIZE] = x[:, :, 1].to(k_pool.dtype)
+    v_pool[slot // PAGE_SIZE, :, slot % PAGE_SIZE] = x[:, :, 2].to(v_pool.dtype)
+
+
+def paged_kv_write(qkv: torch.Tensor, slot: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, D: int) -> None:
+    """Prefill: the keys and values of every token ``n`` of ``qkv [N, n_head*3*D]`` into pool slot ``slot[n]``
+    (``page * PAGE_SIZE + offset``, int32 ``[N]``) for every head.  CUDA bf16 inputs run ``paged_kv_write_kernel``."""
+    if not use_native(qkv):
+        return paged_kv_write_reference(qkv, slot, k_pool, v_pool, D)
+    if D not in DECODE_HEAD_DIMS:
+        raise ValueError(f"the paged KV cache has no head size {D} (supported: {DECODE_HEAD_DIMS})")
+    native().paged_kv_write(qkv.contiguous(), slot.to(torch.int32).contiguous(), k_pool, v_pool)
