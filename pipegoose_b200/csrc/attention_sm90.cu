@@ -21,6 +21,16 @@
 // loop at the block holding the CTA's first query's document start; the backward ends its query loop at the end of the
 // document holding the key block's last key.  Key / query blocks outside those ranges hold no visible pair and are
 // never loaded.  SEG = false compiles to the kernels without the lower bound.
+//
+// Paged prefill (PAGED = true, inference only, no LSE): one CTA per (128-query block, head, sequence r).  The queries
+// are the new tokens cu_seqlens[r] .. cu_seqlens[r+1]-1 of a packed qkv, at positions start[r], start[r]+1, ...; their
+// keys and values are read from the page pools [num_pages, H, 64, D] through the block table, never from qkv, so a
+// cached prefix and the new tokens (already stored by paged_kv_write) are read the same way.  Query at position p sees
+// keys 0 <= k <= p.  A 128-key block is two pages, each loaded as 64-row TMA boxes at an 8 KB offset, which lands in
+// the same swizzled layout as one 128-row box: the consumer loop is shared.  Pool slots past the CTA's last query
+// position may hold anything (NaN included): the second page of the last block is not loaded when it lies wholly
+// past it, and V rows past it are zeroed in shared memory before P.V (a masked p = 0 times NaN would still be NaN).
+// D = 80 runs as D = 128: the pool maps have 80 columns, so TMA's out-of-bounds fill zeroes K / V columns 80..127.
 #include "launch.h"
 #include "pdl_launch.cuh"
 #include "ptx.cuh"
@@ -77,11 +87,18 @@ struct AttFwdArgs {
   int B, S, H, ld_out;
   float scale_log2;  // log2(e) / sqrt(D)
   const int* seg_start;  // [B*S] document start of every token (SEG only)
+  // PAGED only (B = number of sequences, S = max_len, the host bound on new tokens per sequence)
+  const int* cu_seqlens;  // [B+1] rows of each sequence in qkv
+  const int* start;       // [B] position of each sequence's first new token
+  const int* table;       // [B, max_pages] pages of each sequence
+  int max_pages, H_pool;  // table width; heads per page of the pools
+  int d_out;              // columns stored per head (80 for bloom-3b on the D = 128 instantiation)
 };
 
-template <int D, bool SEG>
+template <int D, bool SEG, bool PAGED = false>
 __global__ void __launch_bounds__(kAttThreads, 1)
-    attention_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const AttFwdArgs args) {
+    attention_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const AttFwdArgs args,
+                         const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v) {
   using Cfg = AttFwdCfg<D>;
   constexpr int ST = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -99,12 +116,17 @@ __global__ void __launch_bounds__(kAttThreads, 1)
   const int num_qb = (args.S + ATT_BM - 1) / ATT_BM;
   const int qb = num_qb - 1 - blockIdx.x;  // longest (most key blocks) first
   const int head = blockIdx.y, batch = blockIdx.z;
-  const int num_kb = qb + 1;
-  const int row0 = batch * args.S + qb * ATT_BM;  // global row of the first query
-  const int col_q = head * 3 * D, col_k = col_q + D, col_v = col_q + 2 * D;
+  int num_kb = qb + 1;
+  int row0 = batch * args.S + qb * ATT_BM;  // global row of the first query
+  // (PAGED: qkv's heads are d_out wide, e.g. 80 on the D = 128 instantiation; K / V come from the pools)
+  const int col_q = head * 3 * (PAGED ? args.d_out : D), col_k = col_q + D, col_v = col_q + 2 * D;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tm_qkv);
+    if constexpr (PAGED) {
+      tma_prefetch_desc(&tm_k);
+      tma_prefetch_desc(&tm_v);
+    }
     mbar_init(q_full, 1);
     for (int i = 0; i < ST; ++i) {
       mbar_init(&kv_full[i], 1);
@@ -118,6 +140,17 @@ __global__ void __launch_bounds__(kAttThreads, 1)
   // lowest.  Producer and consumers run the same j0 .. num_kb - 1.
   int j0 = 0;
   if constexpr (SEG) j0 = args.seg_start[row0] / ATT_BN;
+  // PAGED: the sequence's new tokens n_new, the position of the CTA's first query and of its last real one
+  int n_new = 0, p_first = 0, p_last = 0;
+  if constexpr (PAGED) {
+    const int n0 = args.cu_seqlens[batch];
+    n_new = args.cu_seqlens[batch + 1] - n0;
+    if (qb * ATT_BM >= n_new) return;  // past this sequence's end (the grid is sized from the longest)
+    p_first = args.start[batch] + qb * ATT_BM;
+    p_last = args.start[batch] + min(n_new, qb * ATT_BM + ATT_BM) - 1;
+    row0 = n0 + qb * ATT_BM;
+    num_kb = p_last / ATT_BN + 1;
+  }
 
   if (warp < 4) {
     setmaxnreg_dec<kAttRegsLight>();
@@ -132,7 +165,21 @@ __global__ void __launch_bounds__(kAttThreads, 1)
       uint32_t phase = 0;
       for (int j = j0; j < num_kb; ++j) {
         mbar_wait(&kv_empty[stage], phase ^ 1);
-        if (lane == 0) {
+        if (PAGED && lane == 0) {
+          // one 64-row box per page and atom; the second page is skipped when it holds no key <= p_last
+          const int pages = j * ATT_BN + 64 <= p_last ? 2 : 1;
+          const int* trow = args.table + static_cast<size_t>(batch) * args.max_pages + 2 * j;
+          mbar_arrive_expect_tx(&kv_full[stage], pages * Cfg::kTileBytes);
+          for (int pg = 0; pg < pages; ++pg) {
+            const int prow = (trow[pg] * args.H_pool + head) * 64;
+#pragma unroll
+            for (int a = 0; a < D / 64; ++a) {
+              const int off = stage * Cfg::kTileBytes + a * 16384 + pg * 8192;
+              tma_load_2d(sK + off, &tm_k, &kv_full[stage], a * 64, prow);
+              tma_load_2d(sV + off, &tm_v, &kv_full[stage], a * 64, prow);
+            }
+          }
+        } else if (lane == 0) {
           const int krow = batch * args.S + j * ATT_BN;
           mbar_arrive_expect_tx(&kv_full[stage], 2 * Cfg::kTileBytes);
 #pragma unroll
@@ -158,6 +205,14 @@ __global__ void __launch_bounds__(kAttThreads, 1)
   int qpos[2];
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) qpos[hh] = qb * ATT_BM + 64 * wg + 16 * wl + (lane >> 2) + 8 * hh;
+  int qrow[2] = {0, 0};  // PAGED: row index inside the sequence; qpos the position, rows past the end read the last
+  if constexpr (PAGED) {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      qrow[hh] = qpos[hh];
+      qpos[hh] = min(p_first - qb * ATT_BM + qpos[hh], p_last);
+    }
+  }
   const float slope2 = args.slopes[head] * kLog2e;
   int seg[2] = {0, 0};  // document start of each row (padded rows of the last block read the last token's)
   if constexpr (SEG) {
@@ -176,6 +231,21 @@ __global__ void __launch_bounds__(kAttThreads, 1)
   for (int j = j0; j < num_kb; ++j) {
     mbar_wait(&kv_full[stage], phase);
     const uint32_t aK = smem_u32(sK + stage * Cfg::kTileBytes), aV = smem_u32(sV + stage * Cfg::kTileBytes);
+    if constexpr (PAGED) {
+      // V rows past p_last (unwritten slots, or the page that was not loaded) -> 0 before P.V; the two consumer
+      // warpgroups split the rows and meet at a named barrier.  Masked K rows need nothing: their scores become -inf.
+      const int r0 = p_last + 1 - j * ATT_BN;
+      if (r0 < ATT_BN) {
+        uint8_t* v = sV + stage * Cfg::kTileBytes;
+        const int chunks = (ATT_BN - r0) * 8;  // 16-byte chunks per atom
+        for (int c = threadIdx.x - 128; c < chunks * (D / 64); c += 256) {
+          const int a = c / chunks, rc = c - a * chunks;
+          *reinterpret_cast<uint4*>(v + a * 16384 + (r0 + (rc >> 3)) * 128 + (rc & 7) * 16) = make_uint4(0, 0, 0, 0);
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(1, 256);
+      }
+    }
     // S = Q K^T
     wgmma_fence_regs(s);
     wgmma_fence();
@@ -189,7 +259,9 @@ __global__ void __launch_bounds__(kAttThreads, 1)
     wgmma_wait<0>();
     wgmma_fence_regs(s);
     // x = s*scale_log2 + slope2*(kpos - qpos); the causal mask only matters on the diagonal block
-    const bool diag = (j == qb);
+    // (PAGED: query blocks start at start[r], off the key grid; a block holds keys past some query iff its last key
+    // lies past the CTA's first query)
+    const bool diag = PAGED ? (j * ATT_BN + ATT_BN - 1 > p_first) : (j == qb);
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       const float bias0 = slope2 * static_cast<float>(j * ATT_BN - qpos[hh]);
@@ -258,7 +330,16 @@ __global__ void __launch_bounds__(kAttThreads, 1)
     l += __shfl_xor_sync(0xffffffffu, l, 1);
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const float inv_l = 1.f / l;
-    if (qpos[hh] < args.S) {
+    if constexpr (PAGED) {
+      if (qrow[hh] < n_new) {
+        __nv_bfloat16* orow = args.out + static_cast<size_t>(row0 - qb * ATT_BM + qrow[hh]) * args.ld_out + head * args.d_out;
+#pragma unroll
+        for (int jn = 0; jn < D / 8; ++jn)
+          if (8 * jn < args.d_out)
+            *reinterpret_cast<uint32_t*>(orow + 8 * jn + 2 * t4) =
+                pack_bf16x2(o[4 * jn + 2 * hh] * inv_l, o[4 * jn + 2 * hh + 1] * inv_l);
+      }
+    } else if (qpos[hh] < args.S) {
       __nv_bfloat16* orow = args.out + static_cast<size_t>(batch * args.S + qpos[hh]) * args.ld_out + head * D;
 #pragma unroll
       for (int jn = 0; jn < D / 8; ++jn)
@@ -632,7 +713,9 @@ static int launch_att_fwd(const CUtensorMap& tm, const AttFwdArgs& a, cudaStream
     set = true;
   }
   dim3 grid((a.S + ATT_BM - 1) / ATT_BM, a.H, a.B);
-  if (launch_pdl(attention_fwd_kernel<D, SEG>, grid, dim3(kAttThreads), Cfg::kSmemBytes, s, tm, a) != cudaSuccess) return -1;
+  // the pool maps are unused here: the qkv map fills their slots
+  if (launch_pdl(attention_fwd_kernel<D, SEG>, grid, dim3(kAttThreads), Cfg::kSmemBytes, s, tm, a, tm, tm) != cudaSuccess)
+    return -1;
   PG_CHECK_LAUNCH("attention_fwd");
   return 0;
 }
@@ -655,6 +738,54 @@ extern "C" int pg_attention_fwd(const void* qkv, const float* slopes, void* out,
   a.seg_start = seg_start;
   if (seg_start != nullptr) return D == 64 ? launch_att_fwd<64, true>(tm, a, s) : launch_att_fwd<128, true>(tm, a, s);
   return D == 64 ? launch_att_fwd<64, false>(tm, a, s) : launch_att_fwd<128, false>(tm, a, s);
+}
+
+template <int D>
+static int launch_att_fwd_paged(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
+                                const AttFwdArgs& a, cudaStream_t s) {
+  using Cfg = AttFwdCfg<D>;
+  static bool set = false;
+  if (!set) {
+    if (cudaFuncSetAttribute(attention_fwd_kernel<D, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) != cudaSuccess) return -1;
+    set = true;
+  }
+  dim3 grid((a.S + ATT_BM - 1) / ATT_BM, a.H, a.B);
+  if (launch_pdl(attention_fwd_kernel<D, false, true>, grid, dim3(kAttThreads), Cfg::kSmemBytes, s, tq, a, tk, tv) != cudaSuccess)
+    return -1;
+  PG_CHECK_LAUNCH("attention_fwd_paged");
+  return 0;
+}
+
+// Paged prefill attention (PAGED, see the top of the file): qkv [N, H*3*D] holds the new tokens of R sequences
+// (cu_seqlens int32 [R+1], start int32 [R], table int32 [R, max_pages], all on the device); out [N, H*D].  max_len >= the
+// most new tokens of any sequence sizes the grid.  k_pool / v_pool [num_pages, H, 64, D] are read, never written.
+// D = 80 runs on the D = 128 instantiation (pool maps of 80 columns: out-of-bounds columns read as zero).
+extern "C" int pg_paged_prefill_attention(const void* qkv, const void* k_pool, const void* v_pool, const int* table,
+                                          const int* cu_seqlens, const int* start, const float* slopes, void* out, int N,
+                                          int R, int H, int D, int num_pages, int max_pages, int max_len,
+                                          float softmax_scale, cudaStream_t s) {
+  if (D != 64 && D != 80 && D != 128) return -1;
+  if (N <= 0 || R <= 0 || max_len <= 0) return 0;
+  const uint64_t pool_rows = static_cast<uint64_t>(num_pages) * H * 64;
+  if (pool_rows >= (1ull << 31)) return -1;  // TMA row coordinates are int32
+  CUtensorMap tq, tk, tv;
+  if (att_tmap(&tq, qkv, static_cast<uint64_t>(N), static_cast<uint64_t>(H) * 3 * D, ATT_BM) != 0) return -1;
+  if (att_tmap(&tk, k_pool, pool_rows, D, 64) != 0) return -1;
+  if (att_tmap(&tv, v_pool, pool_rows, D, 64) != 0) return -1;
+  AttFwdArgs a;
+  memset(&a, 0, sizeof(a));
+  a.out = (__nv_bfloat16*)out;
+  a.slopes = slopes;
+  a.B = R; a.S = max_len; a.H = H;
+  a.ld_out = H * D;
+  a.scale_log2 = kLog2e * (softmax_scale > 0.f ? softmax_scale : 1.0f / sqrtf(static_cast<float>(D)));
+  a.cu_seqlens = cu_seqlens;
+  a.start = start;
+  a.table = table;
+  a.max_pages = max_pages;
+  a.H_pool = H;
+  a.d_out = D;
+  return D == 64 ? launch_att_fwd_paged<64>(tq, tk, tv, a, s) : launch_att_fwd_paged<128>(tq, tk, tv, a, s);
 }
 
 template <int D, bool SEG>

@@ -417,6 +417,44 @@ void paged_decode_attention(const torch::Tensor& qkv, torch::Tensor k_pool, torc
                                         cur_stream()) == 0, "paged_decode_attention failed");
 }
 
+// Paged prefill attention (attention_sm90.cu, PAGED): the new tokens of R sequences packed in qkv [N, H*3*D] (sequence
+// r: rows cu_seqlens[r] .. cu_seqlens[r+1]-1 at positions start[r], ...) attend to keys 0 .. p of their own sequence,
+// read from the pools through table [R, max_pages]; out [N, H*D].  The pools are not written.  cu_seqlens, start and
+// table stay on the device: the caller guarantees max_len >= every sequence's new tokens, that table[r] holds pages of
+// the pool for positions 0 .. start[r] + new tokens - 1, and that those slots were written.
+void paged_prefill_attention(const torch::Tensor& qkv, const torch::Tensor& k_pool, const torch::Tensor& v_pool,
+                             const torch::Tensor& table, const torch::Tensor& cu_seqlens, const torch::Tensor& start,
+                             int64_t max_len, const torch::Tensor& slopes, torch::Tensor out, double softmax_scale) {
+  check_pools(qkv, k_pool, v_pool, "paged_prefill_attention");
+  PG_CUDA(out); PG_BF16(out); PG_CUDA(slopes); PG_F32(slopes); PG_CUDA(table); PG_CUDA(cu_seqlens); PG_CUDA(start);
+  TORCH_CHECK(table.scalar_type() == torch::kInt32 && cu_seqlens.scalar_type() == torch::kInt32 &&
+              start.scalar_type() == torch::kInt32, "paged_prefill_attention: table, cu_seqlens and start must be int32");
+  TORCH_CHECK(table.dim() == 2 && table.size(1) >= 1 && table.is_contiguous(),
+              "paged_prefill_attention: table must be a contiguous [R, max_pages]");
+  const int64_t R = table.size(0), H = k_pool.size(1), D = k_pool.size(3), max_pages = table.size(1);
+  const int64_t num_pages = k_pool.size(0);
+  TORCH_CHECK(cu_seqlens.numel() == R + 1 && start.numel() == R, "paged_prefill_attention: cu_seqlens must be [R+1] and "
+              "start [R] for the R = ", R, " table rows");
+  TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == H * 3 * D && qkv.is_contiguous(),
+              "paged_prefill_attention: qkv must be a contiguous [N, H*3*D]");
+  const int64_t N = qkv.size(0);
+  TORCH_CHECK(out.numel() == N * H * D && out.is_contiguous() && slopes.numel() == H,
+              "paged_prefill_attention: shape mismatch");
+  TORCH_CHECK(1 <= max_len && max_len <= max_pages * 64, "paged_prefill_attention: max_len ", max_len,
+              " outside 1 .. the ", max_pages * 64, " positions of a table row");
+  TORCH_CHECK(num_pages * H * 64 < (int64_t(1) << 31), "paged_prefill_attention: pools of ", num_pages * H * 64,
+              " rows exceed the 2^31 rows a tensor map addresses");
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&out, &slopes, &table, &cu_seqlens, &start})
+    TORCH_CHECK(t->device() == qkv.device(), "paged_prefill_attention: tensors on different devices");
+  if (N == 0 || R == 0) return;
+  c10::cuda::CUDAGuard guard(qkv.device());
+  TORCH_CHECK(pg_paged_prefill_attention(qkv.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(), table.data_ptr<int>(),
+                                         cu_seqlens.data_ptr<int>(), start.data_ptr<int>(), slopes.data_ptr<float>(),
+                                         out.data_ptr(), (int)N, (int)R, (int)H, (int)D, (int)num_pages,
+                                         (int)max_pages, (int)max_len, (float)softmax_scale, cur_stream()) == 0,
+              "paged_prefill_attention failed");
+}
+
 // Prefill cache write: the k / v of every token n of qkv [N, H*3*D] into pool slot slot[n] (page * 64 + offset).  The
 // caller guarantees every slot lies in the pool.
 void paged_kv_write(const torch::Tensor& qkv, const torch::Tensor& slot, torch::Tensor k_pool, torch::Tensor v_pool) {
@@ -611,6 +649,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("paged_decode_attention", &paged_decode_attention, py::arg("qkv"), py::arg("k_pool"), py::arg("v_pool"),
         py::arg("table"), py::arg("pos"), py::arg("max_pos"), py::arg("slopes"), py::arg("out"), py::arg("ticket"),
         py::arg("softmax_scale") = 0.0);
+  m.def("paged_prefill_attention", &paged_prefill_attention, py::arg("qkv"), py::arg("k_pool"), py::arg("v_pool"),
+        py::arg("table"), py::arg("cu_seqlens"), py::arg("start"), py::arg("max_len"), py::arg("slopes"), py::arg("out"),
+        py::arg("softmax_scale"));
   m.def("paged_kv_write", &paged_kv_write, py::arg("qkv"), py::arg("slot"), py::arg("k_pool"), py::arg("v_pool"));
   m.def("moe_route", &moe_route);
   m.def("moe_dispatch", &moe_dispatch);

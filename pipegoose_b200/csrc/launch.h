@@ -80,6 +80,15 @@ int pg_attention_fwd(const void* qkv, const float* slopes, void* out, float* lse
 int pg_attention_bwd(const void* qkv, const float* slopes, const void* out, const float* lse, const void* dout,
                      void* dqkv, float* dq_acc, float* delta, int B, int S, int H, int D, float softmax_scale,
                      const int* seg_start, cudaStream_t s);
+// Paged prefill: the new tokens of R sequences packed in qkv [N, H*3*D] (sequence r: rows cu_seqlens[r] ..
+// cu_seqlens[r+1]-1 at positions start[r], start[r]+1, ...) attend to keys 0 <= k <= p of their own sequence, all read
+// from k_pool / v_pool [num_pages, H, 64, D] through table [R, max_pages] (the caller stores the new k / v first).
+// cu_seqlens, start, table: int32 on the device; max_len >= every sequence's new tokens (host bound, sizes the grid).
+// out [N, H*D].  D in {64, 80, 128}.  No LSE: inference only.
+int pg_paged_prefill_attention(const void* qkv, const void* k_pool, const void* v_pool, const int* table,
+                               const int* cu_seqlens, const int* start, const float* slopes, void* out, int N, int R,
+                               int H, int D, int num_pages, int max_pages, int max_len, float softmax_scale,
+                               cudaStream_t s);
 
 // ---- decode_sm90.cu
 // One decoding step of B rows at column pos: writes the new k / v of qkv [B, H*3*D] into k_cache / v_cache

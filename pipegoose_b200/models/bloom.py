@@ -658,19 +658,25 @@ class BloomForCausalLM(nn.Module):
     def _paged_logits(self, ids: torch.Tensor, positions: torch.Tensor, k_pools: torch.Tensor, v_pools: torch.Tensor,
                       seg_start: Optional[torch.Tensor] = None, slot: Optional[torch.Tensor] = None,
                       last: Optional[torch.Tensor] = None, table: Optional[torch.Tensor] = None,
-                      max_pos: int = 0) -> torch.Tensor:
+                      max_pos: int = 0, cu_seqlens: Optional[torch.Tensor] = None,
+                      start: Optional[torch.Tensor] = None, max_len: int = 0) -> torch.Tensor:
         """Inference-only forward of a set of sequences over paged KV pools (``pipegoose_b200.serving``); ``ids`` and
         ``positions`` (each token's position in its own sequence) are ``[N]``, ``k_pools`` / ``v_pools`` are
-        ``[n_layer, num_pages, n_head, 64, D]``.  Two modes:
+        ``[n_layer, num_pages, n_head, 64, D]``.  Three modes:
 
         - prefill (``seg_start`` given): the prompts packed into one row, each a document of the flash kernel's
           ``seg_start`` (int32 ``[N]``); ``slot`` (int32 ``[N]``) is each token's pool slot (``page * 64 + offset``).
           Returns the logits at the tokens ``last`` (``[n]``, each prompt's last token): ``[n, V]``.
         - decode: one new token per sequence; ``table`` (int32 ``[N, max_pages]``) holds each sequence's pages,
           ``positions`` (int32) its new token's position, ``max_pos >= max(positions)``.  Returns ``[N, V]``.
+        - prefill with cached prefixes (``start`` given): the suffixes of R prompts whose first ``start[r]`` positions
+          are already in the pools, packed back to back (sequence r: tokens ``cu_seqlens[r] .. cu_seqlens[r+1]-1``);
+          ``positions`` are absolute, ``slot`` is each token's pool slot, ``table`` (int32 ``[R, max_pages]``) each
+          sequence's pages and ``max_len >=`` its suffix length.  Every layer stores the new keys and values, then the
+          suffix attends to the whole sequence through the pools.  Returns the logits at ``last``: ``[R, V]``.
 
-        CUDA bf16 models with head size 64, 80 or 128 run the flash / paged decode kernels; otherwise (CPU, fp32, other
-        head sizes) their PyTorch references run."""
+        CUDA bf16 models with head size 64, 80 or 128 run the flash / paged decode / paged prefill kernels; otherwise
+        (CPU, fp32, other head sizes) their PyTorch references run."""
         from pipegoose_b200.ops import attention as A
 
         cfg = self.config
@@ -680,6 +686,7 @@ class BloomForCausalLM(nn.Module):
         native = _native_decode(self.transformer.h[0].self_attention.query_key_value.weight, D)
         write = A.paged_kv_write if native else A.paged_kv_write_reference
         decode = A.alibi_paged_decode_attention if native else A.alibi_paged_decode_attention_reference
+        prefill = A.alibi_paged_prefill_attention if native else A.paged_prefill_attention_fp32
         pos_emb = self.transformer.position_embeddings.weight[positions.long()] if _learned(cfg) else None
 
         def attend(li, attn, qkv):
@@ -688,10 +695,13 @@ class BloomForCausalLM(nn.Module):
             if seg_start is not None:
                 write(qkv, slot, k_pools[li], v_pools[li], D)
                 return A.alibi_attention(qkv, slopes, 1, N, n_head, D, seg_start=seg_start.view(1, N)).view(1, N, -1)
+            if start is not None:
+                write(qkv, slot, k_pools[li], v_pools[li], D)
+                return prefill(qkv, k_pools[li], v_pools[li], table, cu_seqlens, start, max_len, slopes, D).view(1, N, -1)
             return decode(qkv, k_pools[li], v_pools[li], table, positions, max_pos, slopes, D).view(1, N, -1)
 
         x = self._inference_layers(self._inference_embed(ids.view(1, N), pos_emb), attend)[0]
-        return self._inference_head(x if seg_start is None else x[last.long()])
+        return self._inference_head(x if seg_start is None and start is None else x[last.long()])
 
     def _incremental_logits_tp(self, ids: torch.Tensor, cache: list, past: int,
                                lead: Optional[torch.Tensor] = None, capacity: Optional[int] = None) -> torch.Tensor:

@@ -342,3 +342,85 @@ def paged_kv_write(qkv: torch.Tensor, slot: torch.Tensor, k_pool: torch.Tensor, 
     if D not in DECODE_HEAD_DIMS:
         raise ValueError(f"the paged KV cache has no head size {D} (supported: {DECODE_HEAD_DIMS})")
     native().paged_kv_write(qkv.contiguous(), slot.to(torch.int32).contiguous(), k_pool, v_pool)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Prefill against paged pools (prefix caching, ``pipegoose_b200.serving``).
+#
+# ``qkv [N, n_head*3*D]`` holds the new tokens of R sequences packed back to back: sequence r owns rows
+# ``cu_seqlens[r] .. cu_seqlens[r+1]-1`` (int32 ``[R+1]``), and its first new token sits at position ``start[r]`` (int32
+# ``[R]``), so row n is at ``p = start[r] + n - cu_seqlens[r]``.  Its query attends to keys ``0 <= k <= p`` of sequence r,
+# all read from the pools through ``table`` (int32 ``[R, max_pages]``) with ``q.k * scale + slope[head] * (k - p)``: the
+# cached prefix and the new tokens are read the same way, so the caller stores the new keys and values with
+# :func:`paged_kv_write` first.  The op does not write the pools.  ``max_len`` is a host integer ``>= `` every sequence's
+# new tokens: it sizes the kernel's grid only.  The kernel does not read ``cu_seqlens`` / ``start`` on the host and
+# trusts them (as the decode op trusts ``pos``); it checks ``max_len`` against them only when they are host tensors.
+# ---------------------------------------------------------------------------------------------------------------------
+
+def _check_prefill_bounds(cu_seqlens: torch.Tensor, max_len: int, table: torch.Tensor, D: int = 0) -> None:
+    if D and D not in DECODE_HEAD_DIMS:
+        raise ValueError(f"the paged prefill-attention kernel has no head size {D} (supported: {DECODE_HEAD_DIMS})")
+    if not 1 <= max_len <= table.shape[1] * PAGE_SIZE:
+        raise ValueError(f"max_len {max_len} is outside 1 .. the {table.shape[1] * PAGE_SIZE} positions of a table row")
+    if not cu_seqlens.is_cuda and cu_seqlens.numel() > 1:         # host data: checked without a device sync
+        longest = int((cu_seqlens[1:] - cu_seqlens[:-1]).max())
+        if longest > max_len:
+            raise ValueError(f"max_len {max_len} is smaller than the longest sequence ({longest} new tokens)")
+
+
+def alibi_paged_prefill_attention_reference(qkv: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
+                                            table: torch.Tensor, cu_seqlens: torch.Tensor, start: torch.Tensor,
+                                            max_len: int, slopes: torch.Tensor, D: int,
+                                            softmax_scale: float = 0.0) -> torch.Tensor:
+    """fp32 PyTorch form of :func:`alibi_paged_prefill_attention` (CPU path, test oracle).  Reads ``cu_seqlens`` and
+    ``start`` on the host.  No pool slot past a sequence's last position reaches the result."""
+    _check_prefill_bounds(cu_seqlens.cpu(), max_len, table, D)
+    return paged_prefill_attention_fp32(qkv, k_pool, v_pool, table, cu_seqlens, start, max_len, slopes, D,
+                                        softmax_scale)
+
+
+def paged_prefill_attention_fp32(qkv: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, table: torch.Tensor,
+                                 cu_seqlens: torch.Tensor, start: torch.Tensor, max_len: int, slopes: torch.Tensor,
+                                 D: int, softmax_scale: float = 0.0) -> torch.Tensor:
+    """The reference's computation for any head size (the model's path where no kernel has its head size)."""
+    _check_prefill_bounds(cu_seqlens.cpu(), max_len, table)
+    n_head = k_pool.shape[1]
+    N = qkv.shape[0]
+    out = torch.zeros(N, n_head, D, dtype=torch.float32, device=qkv.device)
+    cu, st = cu_seqlens.tolist(), start.tolist()
+    scale = softmax_scale if softmax_scale > 0 else 1.0 / math.sqrt(D)
+    for r in range(len(st)):
+        n0, n1 = cu[r], cu[r + 1]
+        if n1 == n0:
+            continue
+        last = st[r] + n1 - n0 - 1                                   # the sequence's last position
+        pos = torch.tensor([last], device=k_pool.device)
+        k, _ = _paged_keys(k_pool, table[r:r + 1], pos, last + 1)   # [1, H, last+1, D], zero past `last`
+        v, _ = _paged_keys(v_pool, table[r:r + 1], pos, last + 1)
+        q = qkv[n0:n1].view(n1 - n0, n_head, 3, D)[:, :, 0].float().transpose(0, 1).to(k.device)   # [H, n, D]
+        scores = torch.matmul(q, k[0].transpose(-1, -2)) * scale    # [H, n, last+1]
+        qp = torch.arange(st[r], last + 1, device=k.device).view(1, -1, 1)
+        kp = torch.arange(last + 1, device=k.device).view(1, 1, -1)
+        scores = scores + slopes.float().to(k.device).view(n_head, 1, 1) * (kp - qp).float()
+        scores = scores.masked_fill(kp > qp, float("-inf"))
+        out[n0:n1] = torch.matmul(scores.softmax(-1), v[0]).transpose(0, 1).to(out.device)
+    return out.reshape(N, n_head * D).to(qkv.dtype)
+
+
+def alibi_paged_prefill_attention(qkv: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, table: torch.Tensor,
+                                  cu_seqlens: torch.Tensor, start: torch.Tensor, max_len: int, slopes: torch.Tensor,
+                                  D: int, softmax_scale: float = 0.0) -> torch.Tensor:
+    """Attention of the new tokens of R sequences over their paged keys (section comment above): returns
+    ``[N, n_head*D]``.  CUDA bf16 inputs run the paged form of the flash kernel (``csrc/attention_sm90.cu``, D in
+    64 / 80 / 128; D = 80 on the D = 128 instantiation without padded copies)."""
+    if not use_native(qkv):
+        return alibi_paged_prefill_attention_reference(qkv, k_pool, v_pool, table, cu_seqlens, start, max_len, slopes,
+                                                       D, softmax_scale)
+    _check_prefill_bounds(cu_seqlens, max_len, table, D)
+    n_head = k_pool.shape[1]
+    out = torch.empty(qkv.shape[0], n_head * D, dtype=qkv.dtype, device=qkv.device)
+    native().paged_prefill_attention(qkv.contiguous(), k_pool, v_pool, table.to(torch.int32).contiguous(),
+                                     cu_seqlens.to(qkv.device, torch.int32).contiguous(),
+                                     start.to(qkv.device, torch.int32).contiguous(), int(max_len),
+                                     slopes.float().contiguous(), out, softmax_scale)
+    return out

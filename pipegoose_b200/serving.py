@@ -16,9 +16,24 @@ through the paged split-KV decode kernel.  Tokens are chosen with the model's ``
 requests that share sampling parameters.  A step makes one host-to-device upload (tokens, positions and page tables,
 shared by all layers) and one device-to-host transfer (the chosen tokens).
 
+Prefix caching (``prefix_caching=True``, off by default): full pages of prompts (and, once a request finishes, of its
+generated tokens) stay indexed by their content after use, so a later prompt that starts with the same tokens reuses
+them instead of computing them again.  The key of page k of a sequence is (key id of page k-1, its 64 token ids):
+matching compares token ids exactly.  A request matches its prompt page by page, at most ``(prompt - 1) // 64`` pages
+(its last prompt token is always computed: the step needs its logits), and takes a reference on every hit.  Pages are
+reference-counted; at zero a page returns to the free list but keeps its index entry until it is handed out again,
+least recently freed first (a finished request releases its last page first, so a chain's tail is evicted before its
+prefix).  Invariant: only full pages are shared, and a request never writes into a shared page (its first computed
+position is a page boundary, and decoding writes past the prompt), so no page is ever copied.  A prefill step in which
+some request has a hit runs every request through the paged prefill kernel over the pools (a request without one
+from position 0); otherwise the flash-kernel path above runs.  ``cached_prompt_tokens`` counts the prompt tokens served
+from the cache.  With prefix caching a request's tokens can depend, at rounding level, on which earlier requests left
+pages behind.
+
 Limits: sampled tokens depend on which requests share a step (the random stream is consumed per group);
-an ``ExpertLayer`` capacity limit counts the tokens of one step, as in ``generate()``.  Tensor-parallel, pipelined and
-fused NVLink MoE models are refused.
+an ``ExpertLayer`` capacity limit counts the tokens of one step, as in ``generate()`` (with prefix caching, cached keys
+and values were computed in another step, so with a limit that binds they can differ from a recomputation by more than
+rounding).  Tensor-parallel, pipelined and fused NVLink MoE models are refused.
 """
 from __future__ import annotations
 
@@ -41,6 +56,7 @@ class _Request:
     sampling: Tuple            # (do_sample, temperature, top_k, top_p): requests with the same tuple are picked together
     eos_token_id: Optional[int]
     pages: List[int] = field(default_factory=list)
+    cached: int = 0            # prompt positions served from the prefix cache (a multiple of the page size)
 
     @property
     def pages_needed(self) -> int:
@@ -51,11 +67,13 @@ class ContinuousBatcher:
     """Continuous-batching generation for a ``BloomForCausalLM`` / ``GPT2LMHeadModel`` (module docstring).
 
     ``max_cache_tokens``: KV-cache positions the pools hold (rounded down to whole pages of 64).
-    ``max_prefill_tokens``: most prompt tokens packed into one prefill step.
-    ``generator``: random stream of sampled requests."""
+    ``max_prefill_tokens``: most prompt tokens packed into one prefill step (tokens served from the prefix cache do
+    not count).
+    ``generator``: random stream of sampled requests.
+    ``prefix_caching``: reuse the pages of earlier prompts that share a prefix (module docstring)."""
 
     def __init__(self, model, max_cache_tokens: int, max_prefill_tokens: int = 8192,
-                 generator: Optional[torch.Generator] = None):
+                 generator: Optional[torch.Generator] = None, prefix_caching: bool = False):
         from pipegoose_b200.models.bloom import BloomMLP, _decodes_incrementally
 
         if getattr(model, "tp", None) is not None:
@@ -84,6 +102,15 @@ class ContinuousBatcher:
         self.v_pools = torch.empty(shape, dtype=w.dtype, device=w.device)
         self.device = w.device
         self._free = collections.deque(range(self.num_pages))
+        self.prefix_caching = bool(prefix_caching)
+        self.cached_prompt_tokens = 0                             # prompt tokens served from the prefix cache
+        if self.prefix_caching:
+            # free pages in the order they were freed, O(1) removal of a revived one
+            self._free = collections.OrderedDict.fromkeys(range(self.num_pages))
+            self._refs = [0] * self.num_pages
+            self._index: Dict[Tuple[int, Tuple[int, ...]], int] = {}    # (parent key id, 64 tokens) -> page
+            self._page_key: Dict[int, Tuple[Tuple[int, Tuple[int, ...]], int]] = {}   # page -> (key, key id)
+            self._key_ids = itertools.count()
         self._ids = itertools.count()
         self._waiting: collections.deque = collections.deque()    # submitted, no pages yet
         self._admitted: collections.deque = collections.deque()   # pages reserved, prompt not yet run
@@ -125,7 +152,10 @@ class ContinuousBatcher:
         for r, t in zip(reqs, chosen):
             r.tokens.append(t)
             if len(r.tokens) - r.prompt_len == r.max_new_tokens or t == r.eos_token_id:
-                self._free.extend(r.pages)
+                if self.prefix_caching:
+                    self._release(r)
+                else:
+                    self._free.extend(r.pages)
                 r.pages = []
                 done.append((r.rid, r.tokens))
             else:
@@ -141,12 +171,80 @@ class ContinuousBatcher:
 
     # ------------------------------------------------------------------ internals
     def _admit(self) -> None:
+        if self.prefix_caching:
+            return self._admit_cached()
         while self._waiting and self._waiting[0].pages_needed <= len(self._free):
             r = self._waiting.popleft()
             r.pages = [self._free.popleft() for _ in range(r.pages_needed)]
             if not all(0 <= p < self.num_pages for p in r.pages):
                 raise RuntimeError(f"page ids {r.pages} outside the pool of {self.num_pages} pages")
             self._admitted.append(r)
+
+    # ------------------------------------------------------------------ prefix cache
+    def _match(self, r: _Request) -> List[int]:
+        """Indexed pages holding the prompt's leading full pages, at most ``(prompt - 1) // 64``."""
+        hits, parent = [], -1
+        for k in range((r.prompt_len - 1) // PAGE_SIZE):
+            page = self._index.get((parent, tuple(r.tokens[k * PAGE_SIZE:(k + 1) * PAGE_SIZE])))
+            if page is None:
+                break
+            hits.append(page)
+            parent = self._page_key[page][1]
+        return hits
+
+    def _admit_cached(self) -> None:
+        """First come, first served; hit pages on the free list count against the free pages they are taken from."""
+        while self._waiting:
+            r = self._waiting[0]
+            hits = self._match(r)
+            revived = sum(1 for p in hits if self._refs[p] == 0)
+            if r.pages_needed - len(hits) > len(self._free) - revived:
+                return
+            self._waiting.popleft()
+            for p in hits:
+                if self._refs[p] == 0:
+                    del self._free[p]
+                self._refs[p] += 1
+            fresh = []
+            for _ in range(r.pages_needed - len(hits)):
+                p = self._free.popitem(last=False)[0]                    # least recently freed
+                entry = self._page_key.pop(p, None)
+                if entry is not None:                                    # evicted: its content is about to change
+                    del self._index[entry[0]]
+                self._refs[p] = 1
+                fresh.append(p)
+            r.pages = hits + fresh
+            r.cached = len(hits) * PAGE_SIZE
+            if not all(0 <= p < self.num_pages for p in r.pages):
+                raise RuntimeError(f"page ids {r.pages} outside the pool of {self.num_pages} pages")
+            self._admitted.append(r)
+
+    def _register(self, r: _Request, filled: int) -> None:
+        """Index the request's full pages among positions ``0 .. filled-1`` (all written to the pools).  A key that is
+        already indexed keeps its first page; the chain continues from that page's key id."""
+        parent = -1
+        for k in range(filled // PAGE_SIZE):
+            page = r.pages[k]
+            entry = self._page_key.get(page)
+            if entry is None:
+                key = (parent, tuple(r.tokens[k * PAGE_SIZE:(k + 1) * PAGE_SIZE]))
+                first = self._index.get(key)
+                if first is not None:
+                    entry = self._page_key[first]
+                else:
+                    entry = (key, next(self._key_ids))
+                    self._index[key] = page
+                    self._page_key[page] = entry
+            parent = entry[1]
+
+    def _release(self, r: _Request) -> None:
+        """A finished request: index the pages its generated tokens filled (positions up to ``len(tokens) - 2`` are in
+        the cache), then drop its references, last page first."""
+        self._register(r, len(r.tokens) - 1)
+        for p in reversed(r.pages):
+            self._refs[p] -= 1
+            if self._refs[p] == 0:
+                self._free[p] = None
 
     def _upload(self, rows: List[List[int]]) -> List[torch.Tensor]:
         """Host int lists -> int32 device tensors, in one copy."""
@@ -158,23 +256,18 @@ class ContinuousBatcher:
         next-token logits ``[len(reqs), V]``."""
         if self._admitted:                                      # prefill the oldest admitted prompts
             reqs, n = [], 0
-            while self._admitted and (not reqs or n + self._admitted[0].prompt_len <= self.max_prefill_tokens):
+            while self._admitted and (not reqs or n + self._admitted[0].prompt_len - self._admitted[0].cached
+                                      <= self.max_prefill_tokens):
                 reqs.append(self._admitted.popleft())
-                n += reqs[-1].prompt_len
+                n += reqs[-1].prompt_len - reqs[-1].cached
             reqs.sort(key=lambda r: r.sampling)
-            ids, positions, seg, slot, last, o = [], [], [], [], [], 0
-            for r in reqs:
-                P = r.prompt_len
-                ids += r.tokens
-                positions += range(P)
-                seg += [o] * P
-                slot += [r.pages[p // PAGE_SIZE] * PAGE_SIZE + p % PAGE_SIZE for p in range(P)]
-                o += P
-                last.append(o - 1)
-            ids, positions, seg, slot, last = self._upload([ids, positions, seg, slot, last])
-            logits = self.model._paged_logits(ids, positions, self.k_pools, self.v_pools, seg_start=seg, slot=slot,
-                                              last=last)
-            return reqs, logits.float()
+            if self.prefix_caching:
+                logits = self._prefill_cached(reqs) if any(r.cached for r in reqs) else self._prefill(reqs)
+                for r in reqs:
+                    self.cached_prompt_tokens += r.cached
+                    self._register(r, r.prompt_len)
+                return reqs, logits.float()
+            return reqs, self._prefill(reqs).float()
         reqs = sorted(self._running, key=lambda r: r.sampling)
         self._running = []
         if not reqs:
@@ -186,6 +279,42 @@ class ContinuousBatcher:
         logits = self.model._paged_logits(ids, positions, self.k_pools, self.v_pools, table=table.view(len(reqs), width),
                                           max_pos=max(pos))
         return reqs, logits.float()
+
+    def _prefill(self, reqs: List[_Request]) -> torch.Tensor:
+        """Whole prompts packed into one row through the document-masked flash kernel."""
+        ids, positions, seg, slot, last, o = [], [], [], [], [], 0
+        for r in reqs:
+            P = r.prompt_len
+            ids += r.tokens
+            positions += range(P)
+            seg += [o] * P
+            slot += [r.pages[p // PAGE_SIZE] * PAGE_SIZE + p % PAGE_SIZE for p in range(P)]
+            o += P
+            last.append(o - 1)
+        ids, positions, seg, slot, last = self._upload([ids, positions, seg, slot, last])
+        return self.model._paged_logits(ids, positions, self.k_pools, self.v_pools, seg_start=seg, slot=slot,
+                                        last=last)
+
+    def _prefill_cached(self, reqs: List[_Request]) -> torch.Tensor:
+        """The prompts' uncached suffixes, packed back to back, through the paged prefill kernel over the pools."""
+        ids, positions, slot, last, cu, start, o = [], [], [], [], [0], [], 0
+        width = max(len(r.pages) for r in reqs)
+        table = []
+        for r in reqs:
+            P, st = r.prompt_len, r.cached
+            ids += r.tokens[st:P]
+            positions += range(st, P)
+            slot += [r.pages[p // PAGE_SIZE] * PAGE_SIZE + p % PAGE_SIZE for p in range(st, P)]
+            o += P - st
+            last.append(o - 1)
+            cu.append(o)
+            start.append(st)
+            table += r.pages + [0] * (width - len(r.pages))
+        max_len = max(r.prompt_len - r.cached for r in reqs)
+        ids, positions, slot, last, cu, start, table = self._upload([ids, positions, slot, last, cu, start, table])
+        return self.model._paged_logits(ids, positions, self.k_pools, self.v_pools, slot=slot, last=last,
+                                        table=table.view(len(reqs), width), cu_seqlens=cu, start=start,
+                                        max_len=max_len)
 
     def _select(self, reqs: List[_Request], logits: torch.Tensor) -> List[int]:
         """Next token of every request (``reqs`` grouped by sampling parameters), one device-to-host transfer."""
