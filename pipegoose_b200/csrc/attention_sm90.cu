@@ -10,11 +10,13 @@
 // accumulator fragment of S is the A fragment of P).  [S, S] never exists.
 //
 // Backward: one CTA per (128-key block, head, batch) looping over the 64-row query blocks at or below
-// the diagonal.  Two consumer warpgroups own 64 keys each: S^T = K Q^T and dP^T = V dO^T on the tensor
-// cores, P^T / dS^T recomputed in registers, dV += P^T dO and dK += dS^T Q with P^T / dS^T as register
-// A operands (dV, dK accumulate in registers across the loop), and the warpgroup's share of
-// dQ = dS K (its 64 keys) from dS^T staged in shared memory, reduced into an fp32 buffer with
-// red.global.add.
+// the diagonal.  A pre-kernel writes each query's (lse * log2e, -delta * scale) pair and zeroes
+// the fp32 dQ buffer; the TMA warp loads a query block's pairs next to its Q and dO.  Two consumer
+// warpgroups own 64 keys each: S^T = K Q^T and dP^T = V dO^T on the tensor cores, P^T / dS^T
+// recomputed in registers, dV += P^T dO and dK += dS^T Q with P^T / dS^T as register A operands
+// (dV, dK accumulate in registers across the loop).  dS^T of all 128 keys is staged in shared memory
+// and each warpgroup computes half of dQ = dS K by output columns, contracting over all 128 keys; its
+// fp32 tile goes through shared memory and one thread adds it into the dQ buffer with a TMA reduce.
 //
 // Packed sequences (SEG = true): seg_start[b*S + s] is the row-relative position where the document holding token s
 // begins (non-decreasing along a row), and query q sees key k iff seg_start[q] <= k <= q.  The forward starts its key
@@ -44,6 +46,7 @@ namespace pg {
 
 int make_tmap_bf16_2d(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld,
                       uint32_t box_rows, uint32_t box_cols);
+int make_tmap_f32_3d(CUtensorMap* out, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t box1);
 
 constexpr int ATT_BM = 128;      // queries per forward CTA
 constexpr int ATT_BN = 128;      // keys per block
@@ -55,10 +58,6 @@ PG_DEVICE float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-
-PG_DEVICE void red_add_v2_f32(float* addr, float a, float b) {
-  asm volatile("red.relaxed.gpu.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
 // A operand (k16 slice kk) of a bf16 product from an fp32 accumulator fragment (columns 16 kk .. 16 kk + 15)
@@ -355,12 +354,16 @@ __global__ void __launch_bounds__(kAttThreads, 1)
 // -----------------------------------------------------------------------------------------------
 // backward
 // -----------------------------------------------------------------------------------------------
-// delta[b,h,i] = sum_d dO[i,d] * O[i,d].  One warp per token row: every lane loads 16-byte chunks of the
-// [H*D] row (fully coalesced), the D/8 lanes that share a head reduce with shuffles.
-__global__ void __launch_bounds__(256) attention_delta_kernel(const __nv_bfloat16* __restrict__ dout,
-                                                              const __nv_bfloat16* __restrict__ out,
-                                                              float* __restrict__ delta, int B, int S, int H,
-                                                              int D) {
+// Per-query statistics of the backward loop: stats[b,h,i] = (lse[b,h,i] * log2e, -delta[b,h,i] * scale) with
+// delta = sum_d dO[i,d] * O[i,d], rows of S_pad (S rounded up to 64) pairs so that the kernel loads a query block's
+// 512 bytes with one bulk copy (pairs past S are never written; the kernel does not use them).  The same pass zeroes
+// the row's fp32 dQ accumulator.  One warp per token row: every lane loads 16-byte chunks of the [H*D] row (fully
+// coalesced), the D/8 lanes that share a head reduce with shuffles.
+__global__ void __launch_bounds__(256) attention_bwd_prep_kernel(const __nv_bfloat16* __restrict__ dout,
+                                                                 const __nv_bfloat16* __restrict__ out,
+                                                                 const float* __restrict__ lse, float2* __restrict__ stats,
+                                                                 float* __restrict__ dq_acc, int B, int S, int S_pad,
+                                                                 int H, int D, float scale) {
   pdl_launch_dependents();
   pdl_wait();
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -369,6 +372,8 @@ __global__ void __launch_bounds__(256) attention_delta_kernel(const __nv_bfloat1
   const int nchunks = H * cph;
   const __nv_bfloat16* a = dout + static_cast<size_t>(row) * H * D;
   const __nv_bfloat16* b = out + static_cast<size_t>(row) * H * D;
+  float4* dq_row = reinterpret_cast<float4*>(dq_acc + static_cast<size_t>(row) * H * D);
+  for (int c = lane; c < H * D / 4; c += 32) dq_row[c] = make_float4(0.f, 0.f, 0.f, 0.f);
   const int bidx = row / S, spos = row % S;
   for (int c0 = 0; c0 < nchunks; c0 += 32) {
     const int c = c0 + lane;
@@ -385,7 +390,8 @@ __global__ void __launch_bounds__(256) attention_delta_kernel(const __nv_bfloat1
     for (int o = cph >> 1; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     if (c < nchunks && (lane & (cph - 1)) == 0) {
       const int head = c / cph;
-      delta[(static_cast<size_t>(bidx) * H + head) * S + spos] = s;
+      const size_t bh = static_cast<size_t>(bidx) * H + head;
+      stats[bh * S_pad + spos] = make_float2(lse[bh * S + spos] * kLog2e, -s * scale);
     }
   }
 }
@@ -396,34 +402,47 @@ struct AttBwdCfg {
   static constexpr int kQBytes = ATT_BWD_BM * D * 2;  // Q or dO tile: D/64 atoms of [64 queries x 128 B]
   static constexpr int kQStages = 2;
   static constexpr int kdSBytes = ATT_BN * ATT_BWD_BM * 2;  // dS^T [128 keys x 64 queries], one swizzled atom
-  static constexpr int kSmemBytes = 2 * kKVBytes + 2 * kQStages * kQBytes + kdSBytes + 256 + 1024 /*align*/;
+  static constexpr int kdQCols = D / 2;                     // dQ columns per consumer warpgroup
+  static constexpr int kdQBytes = ATT_BWD_BM * kdQCols * 4;  // fp32 [64 queries x D/2]: D/64 boxes of [64 x 32]
+  static constexpr int kStatBytes = ATT_BWD_BM * 8;         // (lse2, nds) of a query block
+  static constexpr int kSegBytes = ATT_BWD_BM * 4;          // seg_start of a query block (SEG)
+  // K, V; Q, dO, the statistics and seg_start per stage; dS^T and the dQ tiles double-buffered (step it uses buffer
+  // it & 1)
+  static constexpr int kSmemBytes = 2 * kKVBytes + kQStages * (2 * kQBytes + kStatBytes + kSegBytes) + 2 * kdSBytes +
+                                    2 * 2 * kdQBytes + 256 + 1024 /*align*/;
+  static_assert(kSmemBytes <= 227 * 1024, "attention backward: shared memory");
 };
 
 struct AttBwdArgs {
-  const float* lse;
-  const float* delta;
+  const float2* stats;      // [B, H, S_pad] (lse * log2e, -delta * scale), see attention_bwd_prep_kernel
   const float* slopes;
-  float* dq_acc;            // [B*S, H*D] fp32, zero-initialised
   __nv_bfloat16* dqkv;      // [B*S, H*3*D]
-  int B, S, H;
+  int B, S, H, S_pad;
   float scale, scale_log2;
   const int* seg_start;     // [B*S] document start of every token (SEG only)
 };
 
+// tm_dq: fp32 map over the zeroed dQ accumulator [B, S, H*D] with [64 x 32] boxes; a box's rows past S are clipped,
+// so no query of the next sequence is touched.
 template <int D, bool SEG>
 __global__ void __launch_bounds__(kAttThreads, 1)
     attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant__ CUtensorMap tm_q,
-                         const __grid_constant__ CUtensorMap tm_do, const AttBwdArgs args) {
+                         const __grid_constant__ CUtensorMap tm_do, const __grid_constant__ CUtensorMap tm_dq,
+                         const AttBwdArgs args) {
   using Cfg = AttBwdCfg<D>;
   constexpr int QS = Cfg::kQStages;
+  constexpr int DQN = Cfg::kdQCols;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* sK = smem;
   uint8_t* sV = sK + Cfg::kKVBytes;
   uint8_t* sQ = sV + Cfg::kKVBytes;
   uint8_t* sdO = sQ + QS * Cfg::kQBytes;
-  uint8_t* sdS = sdO + QS * Cfg::kQBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sdS + Cfg::kdSBytes);
+  uint8_t* sdS = sdO + QS * Cfg::kQBytes;  // [2][kdSBytes]
+  uint8_t* sdQ = sdS + 2 * Cfg::kdSBytes;  // [2 buffers][2 warpgroups][kdQBytes]
+  float2* sStat = reinterpret_cast<float2*>(sdQ + 4 * Cfg::kdQBytes);  // [QS][64]
+  int* sSeg = reinterpret_cast<int*>(sStat + QS * ATT_BWD_BM);         // [QS][64] (SEG)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sSeg + QS * ATT_BWD_BM);
   uint64_t* kv_full = bars;         // 1
   uint64_t* q_full = bars + 1;      // QS
   uint64_t* q_empty = q_full + QS;  // QS
@@ -442,6 +461,7 @@ __global__ void __launch_bounds__(kAttThreads, 1)
     tma_prefetch_desc(&tm_kv);
     tma_prefetch_desc(&tm_q);
     tma_prefetch_desc(&tm_do);
+    tma_prefetch_desc(&tm_dq);
     mbar_init(kv_full, 1);
     for (int i = 0; i < QS; ++i) {
       mbar_init(&q_full[i], 1);
@@ -450,7 +470,7 @@ __global__ void __launch_bounds__(kAttThreads, 1)
     fence_mbar_init();
   }
   __syncthreads();
-  pdl_wait();  // prologue above overlapped the predecessor; Q/K/V, dO, lse, delta are read below
+  pdl_wait();  // prologue above overlapped the predecessor; Q/K/V, dO, the statistics and the zeroed dQ are used below
   if constexpr (SEG) {
     // the last query that sees a key of this block ends the document holding its last key: the first q > k_last with
     // seg_start[q] > k_last, found by binary search over the row's non-decreasing seg_start.  Every thread computes the
@@ -478,18 +498,27 @@ __global__ void __launch_bounds__(kAttThreads, 1)
           tma_load_2d(sV + a * 16384, &tm_kv, kv_full, col_v + a * 64, krow0);
         }
       }
+      const float2* stat_row = args.stats + (static_cast<size_t>(batch) * args.H + head) * args.S_pad;
       int stage = 0;
       uint32_t phase = 0;
       for (int it = 0; it < n_iter; ++it) {
         const int qrow = batch * args.S + (qb0 + it) * ATT_BWD_BM;
         mbar_wait(&q_empty[stage], phase ^ 1);
+        if constexpr (SEG) {
+          // the block's document starts (0 past S), published to the consumers by lane 0's arrive on q_full
+          const int q0 = (qb0 + it) * ATT_BWD_BM;
+          for (int i = lane; i < ATT_BWD_BM; i += 32)
+            st_shared_s32(smem_u32(sSeg + stage * ATT_BWD_BM + i), q0 + i < args.S ? args.seg_start[qrow + i] : 0);
+          __syncwarp();
+        }
         if (lane == 0) {
-          mbar_arrive_expect_tx(&q_full[stage], 2 * Cfg::kQBytes);
+          mbar_arrive_expect_tx(&q_full[stage], 2 * Cfg::kQBytes + Cfg::kStatBytes);
 #pragma unroll
           for (int a = 0; a < D / 64; ++a) {
             tma_load_2d(sQ + stage * Cfg::kQBytes + a * 8192, &tm_q, &q_full[stage], col_q + a * 64, qrow);
             tma_load_2d(sdO + stage * Cfg::kQBytes + a * 8192, &tm_do, &q_full[stage], head * D + a * 64, qrow);
           }
+          bulk_load_1d(sStat + stage * ATT_BWD_BM, stat_row + (qb0 + it) * ATT_BWD_BM, Cfg::kStatBytes, &q_full[stage]);
         }
         __syncwarp();
         if (++stage == QS) {
@@ -513,7 +542,10 @@ __global__ void __launch_bounds__(kAttThreads, 1)
   }
   const float slope2 = args.slopes[head] * kLog2e;
   const uint32_t aK = smem_u32(sK) + wg * 8192, aV = smem_u32(sV) + wg * 8192;
-  const uint32_t adS = smem_u32(sdS);
+  // dQ: this warpgroup's output columns [DQN wg, DQN wg + DQN) of K (MN-major: D/64 atoms 16 KB apart, 2 bytes a column)
+  const uint32_t aKdq = smem_u32(sK) + (wg * DQN / 64) * 16384 + (wg * DQN % 64) * 2;
+  const uint32_t adS0 = smem_u32(sdS), aTile0 = smem_u32(sdQ + wg * Cfg::kdQBytes);
+  const uint32_t aStat0 = smem_u32(sStat) + t4 * 16, aSeg0 = smem_u32(sSeg) + t4 * 8;
   float dv[D / 2], dk[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) {
@@ -548,17 +580,18 @@ __global__ void __launch_bounds__(kAttThreads, 1)
     wgmma_fence_regs(dpt);
     // p = exp2(s*scale_log2 + slope2*(kpos-qpos) - lse2); dS = p * (dP - delta) * scale.  Masked (key after query)
     // and out-of-sequence queries get p = 0.
+    const uint32_t aStat = aStat0 + stage * Cfg::kStatBytes, aSeg = aSeg0 + stage * Cfg::kSegBytes;
 #pragma unroll
     for (int jn = 0; jn < ATT_BWD_BM / 8; ++jn) {
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const int qpos = qb * ATT_BWD_BM + 8 * jn + 2 * t4 + e;
         const bool q_ok = qpos < args.S;
-        const size_t stat_idx = (static_cast<size_t>(batch) * args.H + head) * args.S + qpos;
-        const float lse2 = q_ok ? args.lse[stat_idx] * kLog2e : 0.f;
-        const float nds = q_ok ? -args.delta[stat_idx] * args.scale : 0.f;
+        const float2 sv = ld_shared_v2_f32(aStat + jn * 64 + e * 8);  // (lse2, nds) of query qpos
+        const float lse2 = q_ok ? sv.x : 0.f;
+        const float nds = q_ok ? sv.y : 0.f;
         int seg_q = 0;
-        if constexpr (SEG) seg_q = q_ok ? args.seg_start[static_cast<size_t>(batch) * args.S + qpos] : 0;
+        if constexpr (SEG) seg_q = ld_shared_s32(aSeg + jn * 32 + e * 4);
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
           const int i = 4 * jn + 2 * hh + e;
@@ -571,13 +604,14 @@ __global__ void __launch_bounds__(kAttThreads, 1)
       }
     }
     // dS^T (bf16) -> shared memory, [128 keys x 64 queries] with the 128-byte swizzle, for the dQ product below
+    const uint32_t adS = adS0 + (it & 1) * Cfg::kdSBytes;
 #pragma unroll
     for (int jn = 0; jn < ATT_BWD_BM / 8; ++jn) {
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const int r = kr[hh];
         const uint32_t off = r * 128 + ((jn ^ (r & 7)) << 4) + t4 * 4;
-        *reinterpret_cast<uint32_t*>(sdS + off) = pack_bf16x2(dpt[4 * jn + 2 * hh], dpt[4 * jn + 2 * hh + 1]);
+        st_shared_b32(adS + off, pack_bf16x2(dpt[4 * jn + 2 * hh], dpt[4 * jn + 2 * hh + 1]));
       }
     }
     // dV += P^T dO ; dK += dS^T Q   (contraction over the 64 queries; dO / Q MN-major: D/64 atoms 8 KB apart)
@@ -598,35 +632,48 @@ __global__ void __launch_bounds__(kAttThreads, 1)
       WgmmaRS<D, 1>::mma(dk, dsa[kk], make_wgmma_desc_sw128(aQ + kk * 2048, 8192, 1024), 1u);
     wgmma_commit();
     fence_proxy_async_smem();  // dS^T writes -> async-proxy (wgmma) reads
-    named_bar_sync(2 + wg, 128);
-    // this warpgroup's share of dQ = dS K: its 64 keys, 64 output columns per pass.  A = dS (MN-major: queries
-    // contiguous in the dS^T rows), B = K (MN-major: D contiguous)
+    // this warpgroup's dQ tile buffer was last added by step it - 2: wait until that reduce has read it
+    if (tid_wg == 0) tma_store_wait_read<1>();
+    // both halves of dS^T are written (the other warpgroup last read this buffer in step it - 2, before it arrived
+    // here in step it - 1), and the tile is free
+    named_bar_sync(1, 256);
+    // dQ[:, DQN wg .. + DQN] = dS K over all 128 keys.  A = dS (MN-major: queries contiguous in the dS^T rows),
+    // B = K (MN-major: D contiguous)
+    float dq[DQN / 2];
+    wgmma_fence();
 #pragma unroll
-    for (int pass = 0; pass < D / 64; ++pass) {
-      float dq[32];
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk)
-        Wgmma<64, 1, 1>::mma(dq, make_wgmma_desc_sw128(adS + wg * 8192 + kk * 2048, 8192, 1024),
-                             make_wgmma_desc_sw128(aK + pass * 16384 + kk * 2048, 16384, 1024), kk != 0 ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(dq);
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int qpos = qb * ATT_BWD_BM + 16 * wl + (lane >> 2) + 8 * hh;
-        if (qpos < args.S) {
-          float* dq_row = args.dq_acc + static_cast<size_t>(batch * args.S + qpos) * (args.H * D) + head * D + pass * 64;
-#pragma unroll
-          for (int jn = 0; jn < 8; ++jn) red_add_v2_f32(dq_row + 8 * jn + 2 * t4, dq[4 * jn + 2 * hh], dq[4 * jn + 2 * hh + 1]);
-        }
-      }
-    }
+    for (int kk = 0; kk < ATT_BN / 16; ++kk)
+      Wgmma<DQN, 1, 1>::mma(dq, make_wgmma_desc_sw128(adS + kk * 2048, 8192, 1024),
+                            make_wgmma_desc_sw128(aKdq + kk * 2048, 16384, 1024), kk != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(dq);
     wgmma_fence_regs(dv);
     wgmma_fence_regs(dk);
-    // every wgmma of this step has retired (the waits above cover the dV / dK group): Q / dO / dS^T are free
+    const uint32_t aTile = aTile0 + (it & 1) * 2 * Cfg::kdQBytes;
+    // fp32 tile -> shared memory: D/64 boxes of [64 queries x 32 columns], 128-byte rows with the 128-byte swizzle
+    // (16-byte chunk c of row r at c ^ (r & 7))
+#pragma unroll
+    for (int jn = 0; jn < DQN / 8; ++jn) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = 16 * wl + (lane >> 2) + 8 * hh;
+        const int chunk = 2 * (jn & 3) + (t4 >> 1);
+        const uint32_t off = (jn >> 2) * 8192 + r * 128 + ((chunk ^ (r & 7)) << 4) + (t4 & 1) * 8;
+        st_shared_v2_f32(aTile + off, dq[4 * jn + 2 * hh], dq[4 * jn + 2 * hh + 1]);
+      }
+    }
+    fence_proxy_async_smem();  // tile writes -> async-proxy (TMA) reads
+    // every wgmma of this step has retired (the wait above covers the dV / dK group): Q / dO / the statistics are free
     named_bar_sync(2 + wg, 128);
-    if (tid_wg == 0) mbar_arrive(&q_empty[stage]);
+    if (tid_wg == 0) {
+#pragma unroll
+      for (int b = 0; b < DQN / 32; ++b)
+        tma_reduce_add_3d(&tm_dq, sdQ + ((it & 1) * 2 + wg) * Cfg::kdQBytes + b * 8192, head * D + wg * DQN + b * 32,
+                          qb * ATT_BWD_BM, batch);
+      tma_store_commit();
+      mbar_arrive(&q_empty[stage]);
+    }
     if (++stage == QS) {
       stage = 0;
       phase ^= 1;
@@ -644,6 +691,8 @@ __global__ void __launch_bounds__(kAttThreads, 1)
       *reinterpret_cast<uint32_t*>(dv_row + 8 * jn + 2 * t4) = pack_bf16x2(dv[4 * jn + 2 * hh], dv[4 * jn + 2 * hh + 1]);
     }
   }
+  // the dQ sums are complete (and the tiles read) before the CTA exits, so the convert kernel that follows reads them
+  if (tid_wg == 0) tma_store_wait<0>();
 }
 
 // dq fp32 [rows, H*D] -> bf16 into dqkv[rows, H*3*D] (q slot of every head)
@@ -789,50 +838,62 @@ extern "C" int pg_paged_prefill_attention(const void* qkv, const void* k_pool, c
 }
 
 template <int D, bool SEG>
-static int launch_att_bwd(const CUtensorMap& tkv, const CUtensorMap& tq, const CUtensorMap& tdo, const AttBwdArgs& a,
-                          cudaStream_t s) {
+static int launch_att_bwd(const CUtensorMap& tkv, const CUtensorMap& tq, const CUtensorMap& tdo, const CUtensorMap& tdq,
+                          const AttBwdArgs& a, cudaStream_t s) {
   using Cfg = AttBwdCfg<D>;
   static bool set = false;
   if (!set) {
     if (cudaFuncSetAttribute(attention_bwd_kernel<D, SEG>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) != cudaSuccess) return -1;
     set = true;
   }
+  // key block fastest: the CTAs of one (head, batch) run together and share its Q / dO / statistics reads and dQ
+  // reduce-adds in L2 (with the key block slowest, longest first, the backward measured 12 % slower at D = 64 and
+  // 61 % slower at D = 128 on an H100)
   dim3 grid((a.S + ATT_BN - 1) / ATT_BN, a.H, a.B);
-  if (launch_pdl(attention_bwd_kernel<D, SEG>, grid, dim3(kAttThreads), Cfg::kSmemBytes, s, tkv, tq, tdo, a) != cudaSuccess) return -1;
+  if (launch_pdl(attention_bwd_kernel<D, SEG>, grid, dim3(kAttThreads), Cfg::kSmemBytes, s, tkv, tq, tdo, tdq, a) != cudaSuccess)
+    return -1;
   PG_CHECK_LAUNCH("attention_bwd");
   return 0;
 }
 
-// dq_acc: fp32 workspace [B*S, H*D]; delta: fp32 [B, H, S]
+// dq_acc: fp32 workspace [B*S, H*D] (any contents: the pre-kernel zeroes it); stats: fp32 workspace of
+// pg_attention_bwd_stats_floats(B, S, H) floats
 extern "C" int pg_attention_bwd(const void* qkv, const float* slopes, const void* out, const float* lse,
-                                const void* dout, void* dqkv, float* dq_acc, float* delta, int B, int S, int H,
+                                const void* dout, void* dqkv, float* dq_acc, float* stats, int B, int S, int H,
                                 int D, float softmax_scale, const int* seg_start, cudaStream_t s) {
   if (D != 64 && D != 128) return -1;
   const int64_t rows = static_cast<int64_t>(B) * S;
-  CUtensorMap tkv, tq, tdo;
+  const int S_pad = (S + ATT_BWD_BM - 1) / ATT_BWD_BM * ATT_BWD_BM;
+  CUtensorMap tkv, tq, tdo, tdq;
   if (att_tmap(&tkv, qkv, rows, static_cast<uint64_t>(H) * 3 * D, ATT_BN) != 0) return -1;
   if (att_tmap(&tq, qkv, rows, static_cast<uint64_t>(H) * 3 * D, ATT_BWD_BM) != 0) return -1;
   if (att_tmap(&tdo, dout, rows, static_cast<uint64_t>(H) * D, ATT_BWD_BM) != 0) return -1;
-  if (cudaMemsetAsync(dq_acc, 0, rows * H * D * sizeof(float), s) != cudaSuccess) return -1;
-  {
-    if (launch_pdl(attention_delta_kernel, dim3((unsigned)((rows * 32 + 255) / 256)), dim3(256), 0, s,
-                   (const __nv_bfloat16*)dout, (const __nv_bfloat16*)out, delta, B, S, H, D) != cudaSuccess) return -1;
-    PG_CHECK_LAUNCH("attention_delta");
-  }
+  if (make_tmap_f32_3d(&tdq, dq_acc, static_cast<uint64_t>(H) * D, S, B, ATT_BWD_BM) != 0) return -1;
+  const float scale = softmax_scale > 0.f ? softmax_scale : 1.0f / sqrtf(static_cast<float>(D));
+  if (launch_pdl(attention_bwd_prep_kernel, dim3((unsigned)((rows * 32 + 255) / 256)), dim3(256), 0, s,
+                 (const __nv_bfloat16*)dout, (const __nv_bfloat16*)out, lse, reinterpret_cast<float2*>(stats), dq_acc, B,
+                 S, S_pad, H, D, scale) != cudaSuccess)
+    return -1;
+  PG_CHECK_LAUNCH("attention_bwd_prep");
   AttBwdArgs a;
-  a.lse = lse; a.delta = delta; a.slopes = slopes; a.dq_acc = dq_acc;
+  a.stats = reinterpret_cast<const float2*>(stats);
+  a.slopes = slopes;
   a.dqkv = (__nv_bfloat16*)dqkv;
-  a.B = B; a.S = S; a.H = H;
-  a.scale = softmax_scale > 0.f ? softmax_scale : 1.0f / sqrtf(static_cast<float>(D));
+  a.B = B; a.S = S; a.H = H; a.S_pad = S_pad;
+  a.scale = scale;
   a.scale_log2 = a.scale * kLog2e;
   a.seg_start = seg_start;
   const int rc = seg_start != nullptr
-                     ? (D == 64 ? launch_att_bwd<64, true>(tkv, tq, tdo, a, s) : launch_att_bwd<128, true>(tkv, tq, tdo, a, s))
-                     : (D == 64 ? launch_att_bwd<64, false>(tkv, tq, tdo, a, s) : launch_att_bwd<128, false>(tkv, tq, tdo, a, s));
+                     ? (D == 64 ? launch_att_bwd<64, true>(tkv, tq, tdo, tdq, a, s) : launch_att_bwd<128, true>(tkv, tq, tdo, tdq, a, s))
+                     : (D == 64 ? launch_att_bwd<64, false>(tkv, tq, tdo, tdq, a, s) : launch_att_bwd<128, false>(tkv, tq, tdo, tdq, a, s));
   if (rc != 0) return rc;
   const int64_t total = rows * H * D;
   if (launch_pdl(attention_dq_convert_kernel, dim3((unsigned)((total / 8 + 255) / 256)), dim3(256), 0, s, (const float*)dq_acc,
                  (__nv_bfloat16*)dqkv, (int64_t)rows, H, D) != cudaSuccess) return -1;
   PG_CHECK_LAUNCH("attention_dq_convert");
   return 0;
+}
+
+extern "C" int64_t pg_attention_bwd_stats_floats(int B, int S, int H) {
+  return static_cast<int64_t>(B) * H * ((S + ATT_BWD_BM - 1) / ATT_BWD_BM * ATT_BWD_BM) * 2;
 }

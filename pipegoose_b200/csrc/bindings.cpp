@@ -332,9 +332,9 @@ void attention_bwd(const torch::Tensor& qkv, const torch::Tensor& slopes, const 
   TORCH_CHECK(dout.numel() == out.numel() && dqkv.numel() == qkv.numel(), "attention_bwd: shape mismatch");
   const int* seg = seg_start_ptr(seg_start, qkv, B, S);
   auto dq_acc = torch::empty({B * S, H * D}, qkv.options().dtype(torch::kFloat32));
-  auto delta = torch::empty({B, H, S}, qkv.options().dtype(torch::kFloat32));
+  auto stats = torch::empty({pg_attention_bwd_stats_floats((int)B, (int)S, (int)H)}, qkv.options().dtype(torch::kFloat32));
   TORCH_CHECK(pg_attention_bwd(qkv.data_ptr(), slopes.data_ptr<float>(), out.data_ptr(), lse.data_ptr<float>(), dout.data_ptr(), dqkv.data_ptr(),
-                               dq_acc.data_ptr<float>(), delta.data_ptr<float>(), (int)B, (int)S, (int)H, (int)D, (float)softmax_scale, seg, cur_stream()) == 0, "attention_bwd failed");
+                               dq_acc.data_ptr<float>(), stats.data_ptr<float>(), (int)B, (int)S, (int)H, (int)D, (float)softmax_scale, seg, cur_stream()) == 0, "attention_bwd failed");
 }
 
 // One decoding step (decode_sm90.cu): writes the new k / v of qkv [B, H*3*D] at column pos of k_cache / v_cache

@@ -60,6 +60,27 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t
   return 0;
 }
 
+// 3-D fp32 tensor map over a contiguous [d2, d1, d0] tensor (d0 contiguous) with a [1, box1, 32] box and 128-byte
+// swizzle (32 fp32 = one 128-byte row), for TMA reduce-adds of fp32 tiles.
+int make_tmap_f32_3d(CUtensorMap* out, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint32_t box1) {
+  PFN_encodeTiled enc = get_encode_fn();
+  if (!enc) return -1;
+  cudaFree(nullptr);
+  cuuint64_t dims[3] = {d0, d1, d2};
+  cuuint64_t strides[2] = {d0 * 4, d0 * d1 * 4};
+  cuuint32_t box[3] = {32, box1, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(ptr), dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    fprintf(stderr, "pipegoose_b200: cuTensorMapEncodeTiled (fp32, 3-D) failed (%d) ptr=%p dims=%llu x %llu x %llu\n",
+            (int)r, ptr, (unsigned long long)d0, (unsigned long long)d1, (unsigned long long)d2);
+    return -1;
+  }
+  return 0;
+}
+
 struct TmapKey {
   const void* ptr;
   uint64_t rows, cols, ld;

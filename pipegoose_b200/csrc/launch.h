@@ -77,9 +77,11 @@ typedef struct PgGemmDesc {
 // seg_start: int32 [B*S] row-relative document starts of packed sequences (nullptr: one document per row)
 int pg_attention_fwd(const void* qkv, const float* slopes, void* out, float* lse, int B, int S, int H, int D,
                      float softmax_scale, const int* seg_start, cudaStream_t s);
+// dq_acc: fp32 workspace [B*S, H*D], any contents; stats: fp32 workspace of pg_attention_bwd_stats_floats(B, S, H)
 int pg_attention_bwd(const void* qkv, const float* slopes, const void* out, const float* lse, const void* dout,
-                     void* dqkv, float* dq_acc, float* delta, int B, int S, int H, int D, float softmax_scale,
+                     void* dqkv, float* dq_acc, float* stats, int B, int S, int H, int D, float softmax_scale,
                      const int* seg_start, cudaStream_t s);
+int64_t pg_attention_bwd_stats_floats(int B, int S, int H);
 // Paged prefill: the new tokens of R sequences packed in qkv [N, H*3*D] (sequence r: rows cu_seqlens[r] ..
 // cu_seqlens[r+1]-1 at positions start[r], start[r]+1, ...) attend to keys 0 <= k <= p of their own sequence, all read
 // from k_pool / v_pool [num_pages, H, 64, D] through table [R, max_pages] (the caller stores the new k / v first).

@@ -105,6 +105,15 @@ PG_DEVICE void tma_store_2d(const CUtensorMap* m, const void* smem_src, int32_t 
       "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
       : "memory");
 }
+// 3-D tiled reduce-add shared -> global (bulk group completion, same commit / wait as the store).  The element type
+// of the map selects the add (fp32 for an fp32 map); elements outside the tensor are skipped.
+PG_DEVICE void tma_reduce_add_3d(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1, int32_t c2) {
+  asm volatile(
+      "cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+          reinterpret_cast<uint64_t>(m)),
+      "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
 PG_DEVICE void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 PG_DEVICE void tma_store_wait_read() {
@@ -127,6 +136,26 @@ PG_DEVICE void bulk_store_1d(void* gdst, const void* smem_src, uint32_t bytes) {
                    reinterpret_cast<uint64_t>(gdst)),
                "r"(smem_u32(smem_src)), "r"(bytes)
                : "memory");
+}
+
+// shared-memory access by 32-bit shared address (a generic pointer into dynamic shared memory can compile to a
+// generic LD / ST with 64-bit addresses).  volatile: never moved across the barrier waits around them.
+PG_DEVICE void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+PG_DEVICE void st_shared_v2_f32(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+PG_DEVICE void st_shared_s32(uint32_t addr, int v) { asm volatile("st.shared.s32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+PG_DEVICE int ld_shared_s32(uint32_t addr) {
+  int v;
+  asm volatile("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+PG_DEVICE float2 ld_shared_v2_f32(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
+  return v;
 }
 
 // named barrier over `count` threads (a multiple of 32) of the CTA; id 0 is __syncthreads

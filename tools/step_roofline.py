@@ -46,7 +46,7 @@ def main():
         "GEMM dgrad (NN)": (["gemm_bf16_kernel<256, 0, 1"], gemm_pass, 0, ""),
         "GEMM wgrad (TN, fp32 main-grad accumulate)": (["gemm_bf16_kernel<256, 1, 1"], gemm_pass, 0, ""),
         "attention forward": (["attention_fwd_kernel"], attn_fwd, L * (3 * act + act), "flash, ALiBi in-kernel"),
-        "attention backward (+delta, dQ convert)": (["attention_bwd_kernel", "attention_delta_kernel", "attention_dq_convert_kernel"],
+        "attention backward (+stats, dQ convert)": (["attention_bwd_kernel", "attention_bwd_prep_kernel", "attention_dq_convert_kernel"],
                                                     attn_bwd, L * (3 * act + 2 * act + 3 * act), ""),
         "Adam (fp32 master + 2 moments, bf16 params, fp32 grads)": (["adam_kernel"], 0, n_params * (4 + 8 + 16 + 2), ""),
         "cross entropy (stats + finalize over bf16 logits)": (["ce_finalize_kernel", "ce_stats_kernel"], 0,
