@@ -468,6 +468,98 @@ void paged_kv_write(const torch::Tensor& qkv, const torch::Tensor& slot, torch::
                                 (int)H, (int)D, cur_stream()) == 0, "paged_kv_write failed");
 }
 
+// FP8 pools: e4m3 codes [num_pages, H, 64, D] and fp32 scales [num_pages, H, 64] for K and for V.
+void check_fp8_pools(const torch::Tensor& k_pool, const torch::Tensor& v_pool, const torch::Tensor& k_scales,
+                     const torch::Tensor& v_scales, const torch::Device& device, const char* op) {
+  PG_CUDA(k_pool); PG_CUDA(v_pool); PG_CUDA(k_scales); PG_CUDA(v_scales);
+  TORCH_CHECK(k_pool.scalar_type() == torch::kFloat8_e4m3fn && v_pool.scalar_type() == torch::kFloat8_e4m3fn, op,
+              ": k_pool / v_pool must be float8_e4m3fn");
+  PG_F32(k_scales); PG_F32(v_scales);
+  TORCH_CHECK(k_pool.dim() == 4 && v_pool.sizes() == k_pool.sizes(), op, ": k_pool / v_pool must be [num_pages, H, 64, D]");
+  TORCH_CHECK(k_pool.size(2) == 64, op, ": the pools' page dimension must be 64, got ", k_pool.size(2));
+  const int64_t D = k_pool.size(3);
+  TORCH_CHECK(D == 64 || D == 80 || D == 128, op, ": head size ", D, " has no kernel (64, 80, 128)");
+  TORCH_CHECK(k_scales.sizes() == k_pool.sizes().slice(0, 3) && v_scales.sizes() == k_scales.sizes(), op,
+              ": k_scales / v_scales must be [num_pages, H, 64] like the pools, got ", k_scales.sizes(), " and ",
+              v_scales.sizes());
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&k_pool, &v_pool, &k_scales, &v_scales})
+    TORCH_CHECK(t->device() == device, op, ": tensors on different devices");
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&k_pool, &v_pool})
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, op, ": pools must be 16B aligned");
+}
+
+// paged_kv_write into FP8 pools: every token's k / v quantized into its slot, with their scales.
+void paged_kv_write_fp8(const torch::Tensor& qkv, const torch::Tensor& slot, torch::Tensor k_pool, torch::Tensor v_pool,
+                        torch::Tensor k_scales, torch::Tensor v_scales) {
+  PG_CUDA(qkv); PG_BF16(qkv); PG_CUDA(slot);
+  check_fp8_pools(k_pool, v_pool, k_scales, v_scales, qkv.device(), "paged_kv_write_fp8");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(qkv.data_ptr()) % 16 == 0, "paged_kv_write_fp8: qkv must be 16B aligned");
+  TORCH_CHECK(slot.scalar_type() == torch::kInt32 && slot.device() == qkv.device(), "paged_kv_write_fp8: slot must be int32 on the device of qkv");
+  const int64_t N = slot.numel(), H = k_pool.size(1), D = k_pool.size(3);
+  TORCH_CHECK(qkv.numel() == N * H * 3 * D, "paged_kv_write_fp8: qkv must be [N, H*3*D] for the N = ", N, " slots");
+  c10::cuda::CUDAGuard guard(qkv.device());
+  TORCH_CHECK(pg_paged_kv_write_fp8(qkv.data_ptr(), slot.data_ptr<int>(), k_pool.data_ptr(), v_pool.data_ptr(),
+                                    k_scales.data_ptr<float>(), v_scales.data_ptr<float>(), (int)N, (int)H, (int)D,
+                                    cur_stream()) == 0, "paged_kv_write_fp8 failed");
+}
+
+// paged_decode_attention over FP8 pools.  The key and value at pos[b] enter the attention from qkv, exactly, and are
+// quantized into their slot.
+void paged_decode_attention_fp8(const torch::Tensor& qkv, torch::Tensor k_pool, torch::Tensor v_pool,
+                                torch::Tensor k_scales, torch::Tensor v_scales, const torch::Tensor& table,
+                                const torch::Tensor& pos, int64_t max_pos, const torch::Tensor& slopes, torch::Tensor out,
+                                torch::Tensor ticket, double softmax_scale) {
+  PG_CUDA(qkv); PG_BF16(qkv);
+  check_fp8_pools(k_pool, v_pool, k_scales, v_scales, qkv.device(), "paged_decode_attention_fp8");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(qkv.data_ptr()) % 16 == 0, "paged_decode_attention_fp8: qkv must be 16B aligned");
+  PG_CUDA(out); PG_BF16(out); PG_CUDA(slopes); PG_F32(slopes); PG_CUDA(ticket); PG_CUDA(table); PG_CUDA(pos);
+  TORCH_CHECK(ticket.scalar_type() == torch::kInt32 && table.scalar_type() == torch::kInt32 &&
+              pos.scalar_type() == torch::kInt32, "paged_decode_attention_fp8: ticket, table and pos must be int32");
+  TORCH_CHECK(table.dim() == 2 && table.size(1) >= 1, "paged_decode_attention_fp8: table must be [B, max_pages]");
+  const int64_t B = table.size(0), H = k_pool.size(1), D = k_pool.size(3), max_pages = table.size(1);
+  TORCH_CHECK(pos.numel() == B && qkv.numel() == B * H * 3 * D && out.numel() == B * H * D && slopes.numel() == H,
+              "paged_decode_attention_fp8: shape mismatch");
+  TORCH_CHECK(ticket.numel() >= B * H, "ticket must hold at least B*H = ", B * H, " entries");
+  TORCH_CHECK(0 <= max_pos && max_pos < max_pages * 64, "paged_decode_attention_fp8: max_pos ", max_pos,
+              " outside the ", max_pages, " pages of a table row");
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&out, &slopes, &ticket, &table, &pos})
+    TORCH_CHECK(t->device() == qkv.device(), "paged_decode_attention_fp8: tensors on different devices");
+  if (B == 0) return;
+  c10::cuda::CUDAGuard guard(qkv.device());
+  const int splits = pg_decode_splits((int)B, (int)H, (int)max_pos + 1);
+  torch::Tensor part;
+  if (splits > 1) part = torch::empty({B * H * splits * (D + 2)}, qkv.options().dtype(torch::kFloat32));
+  TORCH_CHECK(pg_paged_decode_attention_fp8(qkv.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(),
+                                            k_scales.data_ptr<float>(), v_scales.data_ptr<float>(), table.data_ptr<int>(),
+                                            pos.data_ptr<int>(), slopes.data_ptr<float>(), out.data_ptr(),
+                                            splits > 1 ? part.data_ptr<float>() : nullptr, ticket.data_ptr<int>(), (int)B,
+                                            (int)H, (int)D, (int)max_pages, (int)max_pos, splits, (float)softmax_scale,
+                                            cur_stream()) == 0, "paged_decode_attention_fp8 failed");
+}
+
+// Pages src[i] (int32 [n]) of the FP8 pools, dequantized, into pages dst[i] of the bf16 pools k_out / v_out
+// [*, H, 64, D].  The caller guarantees that every id is a page of its pool.
+void paged_kv_dequantize(const torch::Tensor& k_pool, const torch::Tensor& v_pool, const torch::Tensor& k_scales,
+                         const torch::Tensor& v_scales, const torch::Tensor& src, const torch::Tensor& dst,
+                         torch::Tensor k_out, torch::Tensor v_out) {
+  check_fp8_pools(k_pool, v_pool, k_scales, v_scales, k_pool.device(), "paged_kv_dequantize");
+  PG_CUDA(src); PG_CUDA(dst); PG_CUDA(k_out); PG_BF16(k_out); PG_CUDA(v_out); PG_BF16(v_out);
+  TORCH_CHECK(src.scalar_type() == torch::kInt32 && dst.scalar_type() == torch::kInt32 && src.numel() == dst.numel(),
+              "paged_kv_dequantize: src and dst must be int32 page lists of one length");
+  TORCH_CHECK(k_out.dim() == 4 && v_out.sizes() == k_out.sizes() && k_out.size(1) == k_pool.size(1) &&
+              k_out.size(2) == 64 && k_out.size(3) == k_pool.size(3),
+              "paged_kv_dequantize: k_out / v_out must be [pages, H, 64, D] like the pools");
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&src, &dst, &k_out, &v_out})
+    TORCH_CHECK(t->device() == k_pool.device(), "paged_kv_dequantize: tensors on different devices");
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&k_out, &v_out})
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, "paged_kv_dequantize: outputs must be 16B aligned");
+  c10::cuda::CUDAGuard guard(k_pool.device());
+  TORCH_CHECK(pg_paged_kv_dequantize(k_pool.data_ptr(), v_pool.data_ptr(), k_scales.data_ptr<float>(),
+                                     v_scales.data_ptr<float>(), src.data_ptr<int>(), dst.data_ptr<int>(),
+                                     k_out.data_ptr(), v_out.data_ptr(), (int)src.numel(), (int)k_pool.size(1),
+                                     (int)k_pool.size(3), cur_stream()) == 0, "paged_kv_dequantize failed");
+}
+
 void moe_route(const torch::Tensor& x, const torch::Tensor& wg, const c10::optional<torch::Tensor>& bg,
                const c10::optional<torch::Tensor>& jitter, int64_t top_k, int64_t capacity, torch::Tensor probs,
                torch::Tensor topk_idx, torch::Tensor topk_prob, torch::Tensor pos, torch::Tensor counts,
@@ -653,6 +745,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("table"), py::arg("cu_seqlens"), py::arg("start"), py::arg("max_len"), py::arg("slopes"), py::arg("out"),
         py::arg("softmax_scale"));
   m.def("paged_kv_write", &paged_kv_write, py::arg("qkv"), py::arg("slot"), py::arg("k_pool"), py::arg("v_pool"));
+  m.def("paged_kv_write_fp8", &paged_kv_write_fp8, py::arg("qkv"), py::arg("slot"), py::arg("k_pool"),
+        py::arg("v_pool"), py::arg("k_scales"), py::arg("v_scales"));
+  m.def("paged_decode_attention_fp8", &paged_decode_attention_fp8, py::arg("qkv"), py::arg("k_pool"),
+        py::arg("v_pool"), py::arg("k_scales"), py::arg("v_scales"), py::arg("table"), py::arg("pos"),
+        py::arg("max_pos"), py::arg("slopes"), py::arg("out"), py::arg("ticket"), py::arg("softmax_scale") = 0.0);
+  m.def("paged_kv_dequantize", &paged_kv_dequantize, py::arg("k_pool"), py::arg("v_pool"), py::arg("k_scales"),
+        py::arg("v_scales"), py::arg("src"), py::arg("dst"), py::arg("k_out"), py::arg("v_out"));
   m.def("moe_route", &moe_route);
   m.def("moe_dispatch", &moe_dispatch);
   m.def("symm_alloc", &symm_alloc);

@@ -111,6 +111,20 @@ int pg_paged_decode_attention(const void* qkv, void* k_pool, void* v_pool, const
 // Prefill: the k / v of every token n of qkv [N, H*3*D] into pool slot slot[n] (page * 64 + offset), all heads.
 int pg_paged_kv_write(const void* qkv, const int* slot, void* k_pool, void* v_pool, int N, int H, int D,
                       cudaStream_t s);
+// FP8 pools: e4m3 codes k_pool / v_pool [num_pages, H, 64, D] with fp32 scales k_scales / v_scales [num_pages, H, 64],
+// one per position and head (value = float(code) * scale).  pg_paged_kv_write_fp8 quantizes every token's k / v into
+// its slot.  pg_paged_decode_attention_fp8 is pg_paged_decode_attention over those pools: the key and value at pos[b]
+// come from qkv exactly and are quantized into their slot.  pg_paged_kv_dequantize writes pages src[i] (int32 [n]) of
+// the FP8 pools, dequantized to bf16, into pages dst[i] of k_out / v_out [*, H, 64, D].
+int pg_paged_kv_write_fp8(const void* qkv, const int* slot, void* k_pool, void* v_pool, float* k_scales,
+                          float* v_scales, int N, int H, int D, cudaStream_t s);
+int pg_paged_decode_attention_fp8(const void* qkv, void* k_pool, void* v_pool, float* k_scales, float* v_scales,
+                                  const int* table, const int* pos, const float* slopes, void* out, float* part,
+                                  int* ticket, int B, int H, int D, int max_pages, int max_pos, int splits,
+                                  float softmax_scale, cudaStream_t s);
+int pg_paged_kv_dequantize(const void* k_pool, const void* v_pool, const float* k_scales, const float* v_scales,
+                           const int* src, const int* dst, void* k_out, void* v_out, int n, int H, int D,
+                           cudaStream_t s);
 
 // ---- moe.cu
 int pg_moe_route(const void* x, const void* wg, const void* bg, const float* jitter, int n, int h, int E, int top_k,

@@ -659,7 +659,9 @@ class BloomForCausalLM(nn.Module):
                       seg_start: Optional[torch.Tensor] = None, slot: Optional[torch.Tensor] = None,
                       last: Optional[torch.Tensor] = None, table: Optional[torch.Tensor] = None,
                       max_pos: int = 0, cu_seqlens: Optional[torch.Tensor] = None,
-                      start: Optional[torch.Tensor] = None, max_len: int = 0) -> torch.Tensor:
+                      start: Optional[torch.Tensor] = None, max_len: int = 0,
+                      k_scales: Optional[torch.Tensor] = None, v_scales: Optional[torch.Tensor] = None,
+                      stage: Optional[tuple] = None) -> torch.Tensor:
         """Inference-only forward of a set of sequences over paged KV pools (``pipegoose_b200.serving``); ``ids`` and
         ``positions`` (each token's position in its own sequence) are ``[N]``, ``k_pools`` / ``v_pools`` are
         ``[n_layer, num_pages, n_head, 64, D]``.  Three modes:
@@ -675,8 +677,13 @@ class BloomForCausalLM(nn.Module):
           sequence's pages and ``max_len >=`` its suffix length.  Every layer stores the new keys and values, then the
           suffix attends to the whole sequence through the pools.  Returns the logits at ``last``: ``[R, V]``.
 
+        FP8 pools (``float8_e4m3fn``) come with fp32 ``k_scales`` / ``v_scales`` ``[n_layer, num_pages, n_head, 64]``;
+        a prefill with cached prefixes then also takes ``stage = (num_pages, src, dst, slot, table)``, the device form of
+        :func:`~pipegoose_b200.ops.attention.fp8_prefill_staging` (``table`` as ``[R, width]``), which the kernel path
+        reads through one bf16 staging pool shared by all layers.
+
         CUDA bf16 models with head size 64, 80 or 128 run the flash / paged decode / paged prefill kernels; otherwise
-        (CPU, fp32, other head sizes) their PyTorch references run."""
+        (CPU, fp32, other head sizes) their PyTorch references run, over FP8 pools too."""
         from pipegoose_b200.ops import attention as A
 
         cfg = self.config
@@ -688,17 +695,28 @@ class BloomForCausalLM(nn.Module):
         decode = A.alibi_paged_decode_attention if native else A.alibi_paged_decode_attention_reference
         prefill = A.alibi_paged_prefill_attention if native else A.paged_prefill_attention_fp32
         pos_emb = self.transformer.position_embeddings.weight[positions.long()] if _learned(cfg) else None
+        staging = None
+        if native and k_scales is not None and start is not None:
+            if stage is None:
+                raise ValueError("a prefill with cached prefixes over FP8 pools needs its staging plan (stage)")
+            shape = (stage[0], n_head, A.PAGE_SIZE, D)
+            w = self.transformer.h[0].self_attention.query_key_value.weight
+            staging = (w.new_empty(shape), w.new_empty(shape)) + tuple(stage[1:])
 
         def attend(li, attn, qkv):
             qkv = qkv.view(N, n_head * 3 * D)
             slopes = attn.alibi_slopes_local(n_head)
+            scales = {} if k_scales is None else {"k_scales": k_scales[li], "v_scales": v_scales[li]}
             if seg_start is not None:
-                write(qkv, slot, k_pools[li], v_pools[li], D)
+                write(qkv, slot, k_pools[li], v_pools[li], D, **scales)
                 return A.alibi_attention(qkv, slopes, 1, N, n_head, D, seg_start=seg_start.view(1, N)).view(1, N, -1)
             if start is not None:
-                write(qkv, slot, k_pools[li], v_pools[li], D)
-                return prefill(qkv, k_pools[li], v_pools[li], table, cu_seqlens, start, max_len, slopes, D).view(1, N, -1)
-            return decode(qkv, k_pools[li], v_pools[li], table, positions, max_pos, slopes, D).view(1, N, -1)
+                write(qkv, slot, k_pools[li], v_pools[li], D, **scales)
+                if staging is not None:
+                    scales["stage"] = staging
+                return prefill(qkv, k_pools[li], v_pools[li], table, cu_seqlens, start, max_len, slopes, D,
+                               **scales).view(1, N, -1)
+            return decode(qkv, k_pools[li], v_pools[li], table, positions, max_pos, slopes, D, **scales).view(1, N, -1)
 
         x = self._inference_layers(self._inference_embed(ids.view(1, N), pos_emb), attend)[0]
         return self._inference_head(x if seg_start is None and start is None else x[last.long()])

@@ -15,6 +15,7 @@ every token, the row-relative position where its document begins.  Query ``q`` t
 from __future__ import annotations
 
 import math
+from typing import Tuple
 
 import torch
 
@@ -259,20 +260,67 @@ def alibi_decode_attention(qkv_new: torch.Tensor, k_cache: torch.Tensor, v_cache
 # keys ``0 <= k <= pos[b]`` with ``q.k * scale + slope[head] * (k - pos[b])``.  ``max_pos`` is a host integer
 # ``>= max(pos)``: it sizes the kernel's grid only.  Neither op reads ``table`` or ``pos`` on the host; their caller
 # guarantees ``pos[b] <= max_pos``, that the pages a row uses are pages of the pool, and that no two rows share one.
+#
+# FP8 pools (``ContinuousBatcher(kv_cache_dtype=torch.float8_e4m3fn)``): the pools hold ``torch.float8_e4m3fn`` codes
+# and every op takes fp32 ``k_scales`` / ``v_scales`` ``[num_pages, n_head, PAGE_SIZE]``, one scale per position and
+# head (:func:`quantize_kv` is the format).  Attention reads positions computed in earlier steps from the FP8 pools,
+# dequantized, and positions computed in the same step from that step's ``qkv``, exactly: the decode op's key at
+# ``pos[b]``, the prefill op's new tokens.
 # ---------------------------------------------------------------------------------------------------------------------
 
 PAGE_SIZE = 64
+FP8_MAX = 448.0                         # largest finite float8_e4m3fn
 
 
-def _paged_keys(pool: torch.Tensor, table: torch.Tensor, pos: torch.Tensor, n: int):
-    """fp32 ``pool`` rows of positions ``0 .. n-1`` of every table row as ``[B, n_head, n, D]``, zero behind
-    ``pos[b]`` (a table row may hold anything behind its last used page, and unwritten slots anything at all), and
-    the mask of the positions ``<= pos[b]``."""
+def quantize_kv(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The FP8 pools' format: ``x [..., D]`` -> (``float8_e4m3fn`` codes ``[..., D]``, fp32 scales ``[...]``).  Per row,
+    ``a = max |x|``, scale ``a / 448`` and codes ``e4m3_rn(x * (448 / a))`` (all 0 when ``a == 0``), in fp32 with IEEE
+    division.  The kernels compute the same bits; no value exceeds 448 after the scaling, so nothing saturates."""
+    x = x.float()
+    a = x.abs().amax(-1, keepdim=True)
+    m = torch.full_like(a, FP8_MAX)       # tensor / tensor: torch computes scalar / tensor as a reciprocal product
+    codes = torch.where(a > 0, x * (m / a), torch.zeros_like(x)).to(torch.float8_e4m3fn)
+    return codes, (a / m).squeeze(-1)
+
+
+def dequantize_kv(codes: torch.Tensor, scales: torch.Tensor) -> torch.Tensor:
+    """fp32 values of FP8 pool rows: ``float(code) * scale``."""
+    return codes.float() * scales.unsqueeze(-1)
+
+
+def _fp8_pools(k_pool: torch.Tensor, k_scales, v_scales) -> bool:
+    """Are these FP8 pools?  They need both scale tensors, and other pools take none."""
+    fp8 = k_pool.dtype == torch.float8_e4m3fn
+    if fp8 != (k_scales is not None) or (k_scales is None) != (v_scales is None):
+        raise ValueError("float8_e4m3fn pools need k_scales and v_scales, and other pools take none")
+    return fp8
+
+
+def _paged_keys(pool: torch.Tensor, table: torch.Tensor, pos: torch.Tensor, n: int, scales=None):
+    """fp32 ``pool`` rows of positions ``0 .. n-1`` of every table row as ``[B, n_head, n, D]`` (dequantized with
+    ``scales`` from FP8 pools), zero behind ``pos[b]`` (a table row may hold anything behind its last used page, and
+    unwritten slots anything at all), and the mask of the positions ``<= pos[b]``."""
     p = torch.arange(n, device=pool.device)
     valid = p.view(1, n) <= pos.view(-1, 1).to(p.dtype)
     pages = torch.where(valid, table.long()[:, p // PAGE_SIZE], torch.zeros_like(valid, dtype=torch.long))
-    rows = pool[pages, :, (p % PAGE_SIZE).view(1, n)].float().masked_fill(~valid.view(*valid.shape, 1, 1), 0.0)
+    slots = (p % PAGE_SIZE).view(1, n)
+    rows = pool[pages, :, slots].float() if scales is None else dequantize_kv(pool[pages, :, slots],
+                                                                              scales[pages, :, slots])
+    rows = rows.masked_fill(~valid.view(*valid.shape, 1, 1), 0.0)
     return rows.transpose(1, 2), valid
+
+
+def _store_kv(k: torch.Tensor, v: torch.Tensor, page: torch.Tensor, off: torch.Tensor, k_pool: torch.Tensor,
+              v_pool: torch.Tensor, k_scales, v_scales) -> None:
+    """``k`` / ``v [n, n_head, D]`` into slot ``off[i]`` of page ``page[i]``, quantized into FP8 pools."""
+    if k_scales is None:
+        k_pool[page, :, off] = k.to(k_pool.dtype)
+        v_pool[page, :, off] = v.to(v_pool.dtype)
+        return
+    for x, pool, scales in ((k, k_pool, k_scales), (v, v_pool, v_scales)):
+        codes, s = quantize_kv(x)
+        pool[page, :, off] = codes.to(pool.device)
+        scales[page, :, off] = s.to(scales.device)
 
 
 def _check_max_pos(max_pos: int, table: torch.Tensor) -> None:
@@ -282,8 +330,10 @@ def _check_max_pos(max_pos: int, table: torch.Tensor) -> None:
 
 def alibi_paged_decode_attention_reference(qkv_new: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
                                            table: torch.Tensor, pos: torch.Tensor, max_pos: int, slopes: torch.Tensor,
-                                           D: int, softmax_scale: float = 0.0) -> torch.Tensor:
+                                           D: int, softmax_scale: float = 0.0, k_scales=None,
+                                           v_scales=None) -> torch.Tensor:
     """fp32 PyTorch form of :func:`alibi_paged_decode_attention` (CPU path, test oracle)."""
+    fp8 = _fp8_pools(k_pool, k_scales, v_scales)
     _check_max_pos(max_pos, table)
     B, n_head = table.shape[0], k_pool.shape[1]
     if B == 0:
@@ -291,10 +341,13 @@ def alibi_paged_decode_attention_reference(qkv_new: torch.Tensor, k_pool: torch.
     x = qkv_new.view(B, n_head, 3, D)
     pos = pos.to(table.device).long()
     page = table.long().gather(1, (pos // PAGE_SIZE).view(B, 1)).view(B)
-    k_pool[page, :, pos % PAGE_SIZE] = x[:, :, 1].to(k_pool.dtype)
-    v_pool[page, :, pos % PAGE_SIZE] = x[:, :, 2].to(v_pool.dtype)
-    k, valid = _paged_keys(k_pool, table, pos, max_pos + 1)
-    v, _ = _paged_keys(v_pool, table, pos, max_pos + 1)
+    _store_kv(x[:, :, 1], x[:, :, 2], page, pos % PAGE_SIZE, k_pool, v_pool, k_scales, v_scales)
+    k, valid = _paged_keys(k_pool, table, pos, max_pos + 1, k_scales)
+    v, _ = _paged_keys(v_pool, table, pos, max_pos + 1, v_scales)
+    if fp8:                                                     # the step's own key and value: exact
+        rows = torch.arange(B, device=k.device)
+        k[rows, :, pos.to(k.device)] = x[:, :, 1].float().to(k.device)
+        v[rows, :, pos.to(k.device)] = x[:, :, 2].float().to(k.device)
     scale = softmax_scale if softmax_scale > 0 else 1.0 / math.sqrt(D)
     scores = torch.einsum("bhd,bhkd->bhk", x[:, :, 0].float(), k) * scale
     key_pos = torch.arange(max_pos + 1, device=k_pool.device)
@@ -306,42 +359,74 @@ def alibi_paged_decode_attention_reference(qkv_new: torch.Tensor, k_pool: torch.
 
 def alibi_paged_decode_attention(qkv_new: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
                                  table: torch.Tensor, pos: torch.Tensor, max_pos: int, slopes: torch.Tensor, D: int,
-                                 softmax_scale: float = 0.0) -> torch.Tensor:
+                                 softmax_scale: float = 0.0, k_scales=None, v_scales=None) -> torch.Tensor:
     """One decoding step of ``B`` independent sequences over the paged pools (section comment above): returns
     ``[B, n_head*D]`` and writes the new keys and values into the pools.  CUDA bf16 inputs run the paged form of the
-    split-KV kernel (``csrc/decode_sm90.cu``, D in 64 / 80 / 128)."""
+    split-KV kernel (``csrc/decode_sm90.cu``, D in 64 / 80 / 128), or its FP8 form over FP8 pools."""
+    fp8 = _fp8_pools(k_pool, k_scales, v_scales)
     if not use_native(qkv_new):
         return alibi_paged_decode_attention_reference(qkv_new, k_pool, v_pool, table, pos, max_pos, slopes, D,
-                                                      softmax_scale)
+                                                      softmax_scale, k_scales=k_scales, v_scales=v_scales)
     if D not in DECODE_HEAD_DIMS:
         raise ValueError(f"the decode-attention kernel has no head size {D} (supported: {DECODE_HEAD_DIMS})")
     _check_max_pos(max_pos, table)
     B, n_head = table.shape[0], k_pool.shape[1]
     out = torch.empty(B, n_head * D, dtype=qkv_new.dtype, device=qkv_new.device)
-    native().paged_decode_attention(qkv_new.contiguous(), k_pool, v_pool, table.to(torch.int32).contiguous(),
-                                    pos.to(torch.int32).contiguous(), int(max_pos), slopes.float().contiguous(), out,
-                                    _decode_ticket(B * n_head, qkv_new.device), softmax_scale)
+    table, pos = table.to(torch.int32).contiguous(), pos.to(torch.int32).contiguous()
+    ticket = _decode_ticket(B * n_head, qkv_new.device)
+    if fp8:
+        native().paged_decode_attention_fp8(qkv_new.contiguous(), k_pool, v_pool, k_scales, v_scales, table, pos,
+                                            int(max_pos), slopes.float().contiguous(), out, ticket, softmax_scale)
+    else:
+        native().paged_decode_attention(qkv_new.contiguous(), k_pool, v_pool, table, pos, int(max_pos),
+                                        slopes.float().contiguous(), out, ticket, softmax_scale)
     return out
 
 
 def paged_kv_write_reference(qkv: torch.Tensor, slot: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
-                             D: int) -> None:
+                             D: int, k_scales=None, v_scales=None) -> None:
     """PyTorch form of :func:`paged_kv_write`."""
+    _fp8_pools(k_pool, k_scales, v_scales)
     n_head = k_pool.shape[1]
     x = qkv.view(-1, n_head, 3, D)
     slot = slot.to(k_pool.device).long()
-    k_pool[slot // PAGE_SIZE, :, slot % PAGE_SIZE] = x[:, :, 1].to(k_pool.dtype)
-    v_pool[slot // PAGE_SIZE, :, slot % PAGE_SIZE] = x[:, :, 2].to(v_pool.dtype)
+    _store_kv(x[:, :, 1], x[:, :, 2], slot // PAGE_SIZE, slot % PAGE_SIZE, k_pool, v_pool, k_scales, v_scales)
 
 
-def paged_kv_write(qkv: torch.Tensor, slot: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, D: int) -> None:
+def paged_kv_write(qkv: torch.Tensor, slot: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, D: int,
+                   k_scales=None, v_scales=None) -> None:
     """Prefill: the keys and values of every token ``n`` of ``qkv [N, n_head*3*D]`` into pool slot ``slot[n]``
-    (``page * PAGE_SIZE + offset``, int32 ``[N]``) for every head.  CUDA bf16 inputs run ``paged_kv_write_kernel``."""
+    (``page * PAGE_SIZE + offset``, int32 ``[N]``) for every head, quantized into FP8 pools.  CUDA bf16 inputs run
+    ``paged_kv_write_kernel`` (``paged_kv_write_fp8_kernel``)."""
+    fp8 = _fp8_pools(k_pool, k_scales, v_scales)
     if not use_native(qkv):
-        return paged_kv_write_reference(qkv, slot, k_pool, v_pool, D)
+        return paged_kv_write_reference(qkv, slot, k_pool, v_pool, D, k_scales, v_scales)
     if D not in DECODE_HEAD_DIMS:
         raise ValueError(f"the paged KV cache has no head size {D} (supported: {DECODE_HEAD_DIMS})")
-    native().paged_kv_write(qkv.contiguous(), slot.to(torch.int32).contiguous(), k_pool, v_pool)
+    if fp8:
+        native().paged_kv_write_fp8(qkv.contiguous(), slot.to(torch.int32).contiguous(), k_pool, v_pool, k_scales,
+                                    v_scales)
+    else:
+        native().paged_kv_write(qkv.contiguous(), slot.to(torch.int32).contiguous(), k_pool, v_pool)
+
+
+def paged_kv_dequantize_reference(k_pool: torch.Tensor, v_pool: torch.Tensor, k_scales: torch.Tensor,
+                                  v_scales: torch.Tensor, src: torch.Tensor, dst: torch.Tensor, k_out: torch.Tensor,
+                                  v_out: torch.Tensor) -> None:
+    """PyTorch form of :func:`paged_kv_dequantize`."""
+    src, dst = src.long().to(k_pool.device), dst.long().to(k_out.device)
+    k_out[dst] = dequantize_kv(k_pool[src], k_scales[src]).to(k_out.dtype).to(k_out.device)
+    v_out[dst] = dequantize_kv(v_pool[src], v_scales[src]).to(v_out.dtype).to(v_out.device)
+
+
+def paged_kv_dequantize(k_pool: torch.Tensor, v_pool: torch.Tensor, k_scales: torch.Tensor, v_scales: torch.Tensor,
+                        src: torch.Tensor, dst: torch.Tensor, k_out: torch.Tensor, v_out: torch.Tensor) -> None:
+    """Pages ``src[i]`` of FP8 pools, dequantized, into pages ``dst[i]`` of ``k_out`` / ``v_out [*, n_head,
+    PAGE_SIZE, D]`` (int32 page lists).  CUDA bf16 outputs run ``kv_dequantize_kernel``."""
+    if not use_native(k_out):
+        return paged_kv_dequantize_reference(k_pool, v_pool, k_scales, v_scales, src, dst, k_out, v_out)
+    native().paged_kv_dequantize(k_pool, v_pool, k_scales, v_scales, src.to(torch.int32).contiguous(),
+                                 dst.to(torch.int32).contiguous(), k_out, v_out)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -355,6 +440,11 @@ def paged_kv_write(qkv: torch.Tensor, slot: torch.Tensor, k_pool: torch.Tensor, 
 # :func:`paged_kv_write` first.  The op does not write the pools.  ``max_len`` is a host integer ``>= `` every sequence's
 # new tokens: it sizes the kernel's grid only.  The kernel does not read ``cu_seqlens`` / ``start`` on the host and
 # trusts them (as the decode op trusts ``pos``); it checks ``max_len`` against them only when they are host tensors.
+#
+# FP8 pools: the new tokens are read from ``qkv`` (the rule of the section above), the cached prefix from the pools.
+# Every cached prefix is a whole number of pages (prefix caching shares full pages only), so the kernel runs on a
+# step-local bf16 staging pool that holds just the step's sequences (:func:`fp8_prefill_staging`): their cached pages
+# dequantized, then their new tokens' exact keys and values.
 # ---------------------------------------------------------------------------------------------------------------------
 
 def _check_prefill_bounds(cu_seqlens: torch.Tensor, max_len: int, table: torch.Tensor, D: int = 0) -> None:
@@ -371,18 +461,19 @@ def _check_prefill_bounds(cu_seqlens: torch.Tensor, max_len: int, table: torch.T
 def alibi_paged_prefill_attention_reference(qkv: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
                                             table: torch.Tensor, cu_seqlens: torch.Tensor, start: torch.Tensor,
                                             max_len: int, slopes: torch.Tensor, D: int,
-                                            softmax_scale: float = 0.0) -> torch.Tensor:
+                                            softmax_scale: float = 0.0, k_scales=None, v_scales=None) -> torch.Tensor:
     """fp32 PyTorch form of :func:`alibi_paged_prefill_attention` (CPU path, test oracle).  Reads ``cu_seqlens`` and
     ``start`` on the host.  No pool slot past a sequence's last position reaches the result."""
     _check_prefill_bounds(cu_seqlens.cpu(), max_len, table, D)
     return paged_prefill_attention_fp32(qkv, k_pool, v_pool, table, cu_seqlens, start, max_len, slopes, D,
-                                        softmax_scale)
+                                        softmax_scale, k_scales=k_scales, v_scales=v_scales)
 
 
 def paged_prefill_attention_fp32(qkv: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, table: torch.Tensor,
                                  cu_seqlens: torch.Tensor, start: torch.Tensor, max_len: int, slopes: torch.Tensor,
-                                 D: int, softmax_scale: float = 0.0) -> torch.Tensor:
+                                 D: int, softmax_scale: float = 0.0, k_scales=None, v_scales=None) -> torch.Tensor:
     """The reference's computation for any head size (the model's path where no kernel has its head size)."""
+    fp8 = _fp8_pools(k_pool, k_scales, v_scales)
     _check_prefill_bounds(cu_seqlens.cpu(), max_len, table)
     n_head = k_pool.shape[1]
     N = qkv.shape[0]
@@ -395,9 +486,13 @@ def paged_prefill_attention_fp32(qkv: torch.Tensor, k_pool: torch.Tensor, v_pool
             continue
         last = st[r] + n1 - n0 - 1                                   # the sequence's last position
         pos = torch.tensor([last], device=k_pool.device)
-        k, _ = _paged_keys(k_pool, table[r:r + 1], pos, last + 1)   # [1, H, last+1, D], zero past `last`
-        v, _ = _paged_keys(v_pool, table[r:r + 1], pos, last + 1)
-        q = qkv[n0:n1].view(n1 - n0, n_head, 3, D)[:, :, 0].float().transpose(0, 1).to(k.device)   # [H, n, D]
+        k, _ = _paged_keys(k_pool, table[r:r + 1], pos, last + 1, k_scales)   # [1, H, last+1, D], zero past `last`
+        v, _ = _paged_keys(v_pool, table[r:r + 1], pos, last + 1, v_scales)
+        x = qkv[n0:n1].view(n1 - n0, n_head, 3, D).float().transpose(0, 1).to(k.device)         # [H, n, 3, D]
+        if fp8:                                                      # the new tokens: exact
+            k[0, :, st[r]:] = x[:, :, 1]
+            v[0, :, st[r]:] = x[:, :, 2]
+        q = x[:, :, 0]
         scores = torch.matmul(q, k[0].transpose(-1, -2)) * scale    # [H, n, last+1]
         qp = torch.arange(st[r], last + 1, device=k.device).view(1, -1, 1)
         kp = torch.arange(last + 1, device=k.device).view(1, 1, -1)
@@ -407,15 +502,48 @@ def paged_prefill_attention_fp32(qkv: torch.Tensor, k_pool: torch.Tensor, v_pool
     return out.reshape(N, n_head * D).to(qkv.dtype)
 
 
+def fp8_prefill_staging(pages, cached, lengths):
+    """Host plan of a prefill with cached prefixes over FP8 pools.  Sequence r has pool pages ``pages[r]``, its first
+    ``cached[r]`` positions (a multiple of PAGE_SIZE) in the pools and ``lengths[r]`` positions in all; it gets staging
+    pages ``o_r .. o_r + ceil(lengths[r] / PAGE_SIZE) - 1``.  Returns ``(num_pages, src, dst, slot, table)``: the
+    staging pool's size, its cached pages' pool ids ``src`` and staging ids ``dst``, the staging slot of every new
+    token (in sequence order) and the staging table rows (int lists, padded with page 0)."""
+    src, dst, slot, rows, o = [], [], [], [], 0
+    for pg, c, n in zip(pages, cached, lengths):
+        if c % PAGE_SIZE:
+            raise ValueError(f"a cached prefix of {c} positions is not a whole number of pages")
+        need = -(-n // PAGE_SIZE)
+        src += pg[:c // PAGE_SIZE]
+        dst += range(o, o + c // PAGE_SIZE)
+        slot += range(o * PAGE_SIZE + c, o * PAGE_SIZE + n)
+        rows.append(list(range(o, o + need)))
+        o += need
+    width = max((len(r) for r in rows), default=1)
+    return o, src, dst, slot, [r + [0] * (width - len(r)) for r in rows]
+
+
 def alibi_paged_prefill_attention(qkv: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, table: torch.Tensor,
                                   cu_seqlens: torch.Tensor, start: torch.Tensor, max_len: int, slopes: torch.Tensor,
-                                  D: int, softmax_scale: float = 0.0) -> torch.Tensor:
+                                  D: int, softmax_scale: float = 0.0, k_scales=None, v_scales=None,
+                                  stage=None) -> torch.Tensor:
     """Attention of the new tokens of R sequences over their paged keys (section comment above): returns
     ``[N, n_head*D]``.  CUDA bf16 inputs run the paged form of the flash kernel (``csrc/attention_sm90.cu``, D in
-    64 / 80 / 128; D = 80 on the D = 128 instantiation without padded copies)."""
+    64 / 80 / 128; D = 80 on the D = 128 instantiation without padded copies).
+
+    Over FP8 pools the kernel reads a bf16 staging pool: ``stage = (k_stage, v_stage, src, dst, slot, table)``, the
+    staging pools ``[>= num_pages, n_head, PAGE_SIZE, D]`` (their content is overwritten) and the device int32 lists
+    of :func:`fp8_prefill_staging` (``table`` as ``[R, width]``).  The reference path needs no ``stage``."""
+    fp8 = _fp8_pools(k_pool, k_scales, v_scales)
     if not use_native(qkv):
         return alibi_paged_prefill_attention_reference(qkv, k_pool, v_pool, table, cu_seqlens, start, max_len, slopes,
-                                                       D, softmax_scale)
+                                                       D, softmax_scale, k_scales=k_scales, v_scales=v_scales)
+    if fp8:
+        if stage is None:
+            raise ValueError("the paged prefill kernel reads FP8 pools through a staging pool: pass stage")
+        k_stage, v_stage, src, dst, slot, table = stage
+        paged_kv_dequantize(k_pool, v_pool, k_scales, v_scales, src, dst, k_stage, v_stage)
+        paged_kv_write(qkv, slot, k_stage, v_stage, D)
+        k_pool, v_pool = k_stage, v_stage
     _check_prefill_bounds(cu_seqlens, max_len, table, D)
     n_head = k_pool.shape[1]
     out = torch.empty(qkv.shape[0], n_head * D, dtype=qkv.dtype, device=qkv.device)

@@ -30,6 +30,16 @@ from position 0); otherwise the flash-kernel path above runs.  ``cached_prompt_t
 from the cache.  With prefix caching a request's tokens can depend, at rounding level, on which earlier requests left
 pages behind.
 
+FP8 KV cache (``kv_cache_dtype=torch.float8_e4m3fn``, off by default): the pools hold one ``float8_e4m3fn`` code per
+element, with fp32 scales ``k_scales`` / ``v_scales [n_layer, num_pages, n_head, 64]``, one per position and head
+(``ops.attention.quantize_kv`` is the format).  The same memory holds about 1.9x the positions.  A step's queries read
+positions computed in earlier steps from the FP8 pools, dequantized, and positions computed in the same step from
+that step's bf16 ``qkv``, exactly.  So a prefill without prefix hits gives the same logits as with default pools (the
+flash kernel runs on ``qkv``; only the cache write quantizes), and a decode step reads its own key exactly.  A
+prefill with hits dequantizes the sequences' cached pages into a bf16 staging pool sized for the step's prompt pages
+and runs the paged prefill kernel on it.  A scale belongs to its page slot, so prefix sharing, reference counting and
+eviction are unchanged.  Accuracy on trained checkpoints is not verified here.
+
 Limits: sampled tokens depend on which requests share a step (the random stream is consumed per group);
 an ``ExpertLayer`` capacity limit counts the tokens of one step, as in ``generate()`` (with prefix caching, cached keys
 and values were computed in another step, so with a limit that binds they can differ from a recomputation by more than
@@ -44,7 +54,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
-from pipegoose_b200.ops.attention import PAGE_SIZE
+from pipegoose_b200.ops.attention import PAGE_SIZE, fp8_prefill_staging
 
 
 @dataclass
@@ -70,10 +80,13 @@ class ContinuousBatcher:
     ``max_prefill_tokens``: most prompt tokens packed into one prefill step (tokens served from the prefix cache do
     not count).
     ``generator``: random stream of sampled requests.
-    ``prefix_caching``: reuse the pages of earlier prompts that share a prefix (module docstring)."""
+    ``prefix_caching``: reuse the pages of earlier prompts that share a prefix (module docstring).
+    ``kv_cache_dtype``: ``None`` keeps the pools in the model's dtype, ``torch.float8_e4m3fn`` stores them in FP8 with
+    per-position scales (module docstring)."""
 
     def __init__(self, model, max_cache_tokens: int, max_prefill_tokens: int = 8192,
-                 generator: Optional[torch.Generator] = None, prefix_caching: bool = False):
+                 generator: Optional[torch.Generator] = None, prefix_caching: bool = False,
+                 kv_cache_dtype: Optional[torch.dtype] = None):
         from pipegoose_b200.models.bloom import BloomMLP, _decodes_incrementally
 
         if getattr(model, "tp", None) is not None:
@@ -85,6 +98,8 @@ class ContinuousBatcher:
         if not all(isinstance(b.mlp, BloomMLP) or _decodes_incrementally(b.mlp) for b in blocks):
             raise ValueError("ContinuousBatcher does not support the fused NVLink MoE layer (its kernels are built "
                              "around token-sharded full sequences); use ExpertLayer MLPs")
+        if kv_cache_dtype not in (None, torch.float8_e4m3fn):
+            raise ValueError(f"kv_cache_dtype must be None or torch.float8_e4m3fn, got {kv_cache_dtype}")
         if max_prefill_tokens < 1:
             raise ValueError(f"max_prefill_tokens must be at least 1, got {max_prefill_tokens}")
         cfg = model.config
@@ -98,8 +113,12 @@ class ContinuousBatcher:
         w = blocks[0].self_attention.query_key_value.weight
         D = cfg.hidden_size // cfg.n_head
         shape = (len(blocks), self.num_pages, cfg.n_head, PAGE_SIZE, D)
-        self.k_pools = torch.empty(shape, dtype=w.dtype, device=w.device)
-        self.v_pools = torch.empty(shape, dtype=w.dtype, device=w.device)
+        self.k_pools = torch.empty(shape, dtype=kv_cache_dtype or w.dtype, device=w.device)
+        self.v_pools = torch.empty(shape, dtype=kv_cache_dtype or w.dtype, device=w.device)
+        self.k_scales = self.v_scales = None
+        if kv_cache_dtype is not None:
+            self.k_scales = torch.empty(shape[:-1], dtype=torch.float32, device=w.device)
+            self.v_scales = torch.empty(shape[:-1], dtype=torch.float32, device=w.device)
         self.device = w.device
         self._free = collections.deque(range(self.num_pages))
         self.prefix_caching = bool(prefix_caching)
@@ -277,7 +296,7 @@ class ContinuousBatcher:
         pos = [len(r.tokens) - 1 for r in reqs]
         ids, positions, table = self._upload([[r.tokens[-1] for r in reqs], pos, table])
         logits = self.model._paged_logits(ids, positions, self.k_pools, self.v_pools, table=table.view(len(reqs), width),
-                                          max_pos=max(pos))
+                                          max_pos=max(pos), k_scales=self.k_scales, v_scales=self.v_scales)
         return reqs, logits.float()
 
     def _prefill(self, reqs: List[_Request]) -> torch.Tensor:
@@ -293,10 +312,11 @@ class ContinuousBatcher:
             last.append(o - 1)
         ids, positions, seg, slot, last = self._upload([ids, positions, seg, slot, last])
         return self.model._paged_logits(ids, positions, self.k_pools, self.v_pools, seg_start=seg, slot=slot,
-                                        last=last)
+                                        last=last, k_scales=self.k_scales, v_scales=self.v_scales)
 
     def _prefill_cached(self, reqs: List[_Request]) -> torch.Tensor:
-        """The prompts' uncached suffixes, packed back to back, through the paged prefill kernel over the pools."""
+        """The prompts' uncached suffixes, packed back to back, through the paged prefill kernel over the pools (over a
+        bf16 staging pool with FP8 pools: its plan goes in the step's upload)."""
         ids, positions, slot, last, cu, start, o = [], [], [], [], [0], [], 0
         width = max(len(r.pages) for r in reqs)
         table = []
@@ -311,10 +331,18 @@ class ContinuousBatcher:
             start.append(st)
             table += r.pages + [0] * (width - len(r.pages))
         max_len = max(r.prompt_len - r.cached for r in reqs)
-        ids, positions, slot, last, cu, start, table = self._upload([ids, positions, slot, last, cu, start, table])
+        rows, stage = [ids, positions, slot, last, cu, start, table], None
+        if self.k_scales is not None:
+            n, src, dst, st_slot, st_table = fp8_prefill_staging([r.pages for r in reqs], [r.cached for r in reqs],
+                                                                 [r.prompt_len for r in reqs])
+            rows += [src, dst, st_slot, [p for row in st_table for p in row]]
+        up = self._upload(rows)
+        ids, positions, slot, last, cu, start, table = up[:7]
+        if self.k_scales is not None:
+            stage = (n, up[7], up[8], up[9], up[10].view(len(reqs), -1))
         return self.model._paged_logits(ids, positions, self.k_pools, self.v_pools, slot=slot, last=last,
                                         table=table.view(len(reqs), width), cu_seqlens=cu, start=start,
-                                        max_len=max_len)
+                                        max_len=max_len, k_scales=self.k_scales, v_scales=self.v_scales, stage=stage)
 
     def _select(self, reqs: List[_Request], logits: torch.Tensor) -> List[int]:
         """Next token of every request (``reqs`` grouped by sampling parameters), one device-to-host transfer."""
