@@ -153,6 +153,8 @@ bool parse_grad_rs(const py::dict& d, PgGradRS* out) {
 #define PG_CUDA(t) TORCH_CHECK((t).is_cuda() && (t).is_contiguous(), #t " must be a contiguous CUDA tensor")
 #define PG_BF16(t) TORCH_CHECK((t).scalar_type() == torch::kBFloat16, #t " must be bf16")
 #define PG_F32(t) TORCH_CHECK((t).scalar_type() == torch::kFloat32, #t " must be fp32")
+#define PG_ALIGNED(t, bytes) \
+  TORCH_CHECK(reinterpret_cast<uintptr_t>((t).data_ptr()) % (bytes) == 0, #t " must be " #bytes "-byte aligned")
 
 const void* opt_ptr(const c10::optional<torch::Tensor>& t) { return t.has_value() ? t->data_ptr() : nullptr; }
 
@@ -201,9 +203,11 @@ void embedding_bwd(const torch::Tensor& dx, const torch::Tensor& ids, torch::Ten
   const int h = (int)dx.size(-1);
   const int rows = (int)(dx.numel() / h);
   TORCH_CHECK(ids.scalar_type() == torch::kInt64 && ids.numel() == rows, "ids must be int64 [rows]");
+  // the kernel adds rows in chunks of 8 columns: any other width would drop the last columns
+  TORCH_CHECK(h % 8 == 0, "embedding_bwd: hidden size must be a multiple of 8");
+  PG_ALIGNED(dx, 16);
   PgGradRS grs;
   const bool inl = parse_grad_rs(grad_rs, &grs);
-  TORCH_CHECK(!inl || h % 8 == 0, "embedding_bwd with grad_rs: hidden size must be a multiple of 8");
   TORCH_CHECK(pg_embedding_bwd(dx.data_ptr(), ids.data_ptr<int64_t>(), dw.data_ptr<float>(), rows, h, (int)vocab_start, (int)vocab_end,
                                inl ? &grs : nullptr, cur_stream()) == 0, "embedding_bwd failed");
 }
@@ -245,8 +249,11 @@ void adam_step(torch::Tensor master, torch::Tensor m, torch::Tensor v, const tor
   c10::cuda::CUDAGuard guard(master.device());
   const int64_t n = master.numel();
   TORCH_CHECK(m.numel() == n && v.numel() == n && grad.numel() == n, "adam: size mismatch");
+  // float4 accesses of the fp32 buffers, 8-byte stores of four bf16 parameters
+  PG_ALIGNED(master, 16); PG_ALIGNED(m, 16); PG_ALIGNED(v, 16); PG_ALIGNED(grad, 16);
   void* pb = nullptr;
-  if (param_bf16.has_value()) { PG_CUDA(*param_bf16); PG_BF16(*param_bf16); TORCH_CHECK(param_bf16->numel() == n, "adam: bf16 param size mismatch"); pb = param_bf16->data_ptr(); }
+  if (param_bf16.has_value()) { PG_CUDA(*param_bf16); PG_BF16(*param_bf16); TORCH_CHECK(param_bf16->numel() == n, "adam: bf16 param size mismatch");
+    PG_ALIGNED(*param_bf16, 8); pb = param_bf16->data_ptr(); }
   const double bc1 = 1.0 - std::pow(beta1, (double)step), bc2 = 1.0 - std::pow(beta2, (double)step);
   TORCH_CHECK(pg_adam(master.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(), grad.data_ptr<float>(), pb, n, (float)lr, (float)beta1, (float)beta2,
                       (float)eps, (float)wd, (float)bc1, (float)bc2, (float)grad_scale, adamw, zero_grad, cur_stream()) == 0, "adam failed");
@@ -261,32 +268,24 @@ void adam_step_strided(torch::Tensor master, torch::Tensor m, torch::Tensor v, t
   c10::cuda::CUDAGuard guard(master.device());
   TORCH_CHECK(master.numel() == seg * nb && m.numel() == seg * nb && v.numel() == seg * nb, "adam_strided: state size mismatch");
   TORCH_CHECK(first >= 0 && first + (nb - 1) * bucket_stride + seg <= flat_grad.numel(), "adam_strided: range outside the flat buffer");
+  // float4 accesses from flat_grad + first (seg and bucket_stride are checked by the launcher), 8-byte parameter stores
+  TORCH_CHECK(first % 4 == 0, "adam_strided: first must be a multiple of 4");
+  PG_ALIGNED(master, 16); PG_ALIGNED(m, 16); PG_ALIGNED(v, 16); PG_ALIGNED(flat_grad, 16);
   void* pb = nullptr;
   if (flat_param.has_value()) { PG_CUDA(*flat_param); PG_BF16(*flat_param); TORCH_CHECK(flat_param->numel() == flat_grad.numel(), "flat sizes differ");
-    pb = reinterpret_cast<char*>(flat_param->data_ptr()) + 2 * first; }
+    PG_ALIGNED(*flat_param, 8); pb = reinterpret_cast<char*>(flat_param->data_ptr()) + 2 * first; }
   const double bc1 = 1.0 - std::pow(beta1, (double)step), bc2 = 1.0 - std::pow(beta2, (double)step);
   TORCH_CHECK(pg_adam_strided(master.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(), flat_grad.data_ptr<float>() + first, pb, seg,
                               bucket_stride, nb, (float)lr, (float)beta1, (float)beta2, (float)eps, (float)wd, (float)bc1, (float)bc2,
                               (float)grad_scale, adamw, zero_grad, cur_stream()) == 0, "adam_strided failed");
 }
 
-void sgd_step(torch::Tensor master, c10::optional<torch::Tensor> mom, const torch::Tensor& grad, c10::optional<torch::Tensor> param_bf16,
-              double lr, double momentum, double wd, double grad_scale, bool first_step) {
-  PG_CUDA(master); PG_F32(master); PG_CUDA(grad); PG_F32(grad);
-  c10::cuda::CUDAGuard guard(master.device());
-  const int64_t n = master.numel();
-  float* mp = nullptr;
-  if (mom.has_value()) { PG_CUDA(*mom); PG_F32(*mom); mp = mom->data_ptr<float>(); }
-  TORCH_CHECK(momentum == 0.0 || mp != nullptr, "sgd: momentum buffer required");
-  void* pb = nullptr;
-  if (param_bf16.has_value()) { PG_CUDA(*param_bf16); PG_BF16(*param_bf16); pb = param_bf16->data_ptr(); }
-  TORCH_CHECK(pg_sgd(master.data_ptr<float>(), mp, grad.data_ptr<float>(), pb, n, (float)lr, (float)momentum, (float)wd, (float)grad_scale, first_step, cur_stream()) == 0, "sgd failed");
-}
-
 void accum_bf16_to_f32(const torch::Tensor& src, torch::Tensor dst, double scale, bool accumulate) {
   PG_CUDA(src); PG_BF16(src); PG_CUDA(dst); PG_F32(dst);
   c10::cuda::CUDAGuard guard(src.device());
   TORCH_CHECK(src.numel() == dst.numel(), "size mismatch");
+  // 16-byte loads of src and float4 stores to dst
+  PG_ALIGNED(src, 16); PG_ALIGNED(dst, 16);
   TORCH_CHECK(pg_accum_bf16_to_f32(src.data_ptr(), dst.data_ptr<float>(), src.numel(), (float)scale, accumulate, cur_stream()) == 0, "accum failed");
 }
 
@@ -729,7 +728,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("wd"), py::arg("step"), py::arg("grad_scale"), py::arg("adamw"),
         py::arg("zero_grad") = false);
   m.def("adam_step_strided", &adam_step_strided);
-  m.def("sgd_step", &sgd_step);
   m.def("accum_bf16_to_f32", &accum_bf16_to_f32);
   m.def("attention_fwd", &attention_fwd, py::arg("qkv"), py::arg("slopes"), py::arg("out"), py::arg("lse"), py::arg("B"),
         py::arg("S"), py::arg("H"), py::arg("D"), py::arg("softmax_scale") = 0.0, py::arg("seg_start") = py::none());

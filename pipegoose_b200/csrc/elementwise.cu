@@ -431,6 +431,20 @@ __global__ void __launch_bounds__(512) ce_finalize_kernel(
 // fused Adam(W) on a flat shard: fp32 master / moments, fp32 grads (already averaged),
 // writes the bf16 model copy.  grad_scale folds in loss-scale / clipping coefficients.
 // ---------------------------------------------------------------------------------------------
+// One element of the step.  Every operation is rounded explicitly, leaving the compiler no multiply-add contraction to
+// choose: adam_kernel's vector and scalar paths and adam_strided_kernel give the same bits for the same inputs.
+__device__ __forceinline__ void adam_update(float& p, float& m, float& v, float g, float lr, float beta1, float beta2,
+                                            float eps, float weight_decay, float bc1, float bc2, float grad_scale,
+                                            int adamw) {
+  g = __fmul_rn(g, grad_scale);
+  if (!adamw && weight_decay != 0.f) g = __fmaf_rn(weight_decay, p, g);
+  m = __fmaf_rn(beta1, m, __fmul_rn(__fsub_rn(1.f, beta1), g));
+  v = __fmaf_rn(beta2, v, __fmul_rn(__fmul_rn(__fsub_rn(1.f, beta2), g), g));
+  const float denom = __fadd_rn(__fsqrt_rn(__fdiv_rn(v, bc2)), eps);
+  if (adamw && weight_decay != 0.f) p = __fmul_rn(p, __fsub_rn(1.f, __fmul_rn(lr, weight_decay)));
+  p = __fsub_rn(p, __fdiv_rn(__fmul_rn(lr, __fdiv_rn(m, bc1)), denom));
+}
+
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ master,
                                                    float* __restrict__ exp_avg,
                                                    float* __restrict__ exp_avg_sq,
@@ -452,15 +466,8 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ master,
     float pp[4] = {p.x, p.y, p.z, p.w}, mm[4] = {m.x, m.y, m.z, m.w}, vv[4] = {v.x, v.y, v.z, v.w};
     const float gg[4] = {g4.x, g4.y, g4.z, g4.w};
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float g = gg[j] * grad_scale;
-      if (!adamw && weight_decay != 0.f) g += weight_decay * pp[j];
-      mm[j] = beta1 * mm[j] + (1.f - beta1) * g;
-      vv[j] = beta2 * vv[j] + (1.f - beta2) * g * g;
-      const float denom = sqrtf(vv[j] / bc2) + eps;
-      if (adamw && weight_decay != 0.f) pp[j] *= (1.f - lr * weight_decay);
-      pp[j] -= lr * (mm[j] / bc1) / denom;
-    }
+    for (int j = 0; j < 4; ++j)
+      adam_update(pp[j], mm[j], vv[j], gg[j], lr, beta1, beta2, eps, weight_decay, bc1, bc2, grad_scale, adamw);
     *reinterpret_cast<float4*>(master + i4) = make_float4(pp[0], pp[1], pp[2], pp[3]);
     *reinterpret_cast<float4*>(exp_avg + i4) = make_float4(mm[0], mm[1], mm[2], mm[3]);
     *reinterpret_cast<float4*>(exp_avg_sq + i4) = make_float4(vv[0], vv[1], vv[2], vv[3]);
@@ -470,13 +477,8 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ master,
     }
   } else {
     for (int64_t i = i4; i < n; ++i) {
-      float g = grad[i] * grad_scale;
-      float p = master[i];
-      if (!adamw && weight_decay != 0.f) g += weight_decay * p;
-      const float m = beta1 * exp_avg[i] + (1.f - beta1) * g;
-      const float v = beta2 * exp_avg_sq[i] + (1.f - beta2) * g * g;
-      if (adamw && weight_decay != 0.f) p *= (1.f - lr * weight_decay);
-      p -= lr * (m / bc1) / (sqrtf(v / bc2) + eps);
+      float p = master[i], m = exp_avg[i], v = exp_avg_sq[i];
+      adam_update(p, m, v, grad[i], lr, beta1, beta2, eps, weight_decay, bc1, bc2, grad_scale, adamw);
       master[i] = p;
       exp_avg[i] = m;
       exp_avg_sq[i] = v;
@@ -484,27 +486,6 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ master,
       if (zero_grad) const_cast<float*>(grad)[i] = 0.f;
     }
   }
-}
-
-// SGD (+momentum) on a flat shard, same conventions.
-__global__ void __launch_bounds__(256) sgd_kernel(float* __restrict__ master, float* __restrict__ mom,
-                                                  const float* __restrict__ grad,
-                                                  __nv_bfloat16* __restrict__ param_bf16, int64_t n,
-                                                  float lr, float momentum, float weight_decay,
-                                                  float grad_scale, int first_step) {
-  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float g = grad[i] * grad_scale;
-  float p = master[i];
-  if (weight_decay != 0.f) g += weight_decay * p;
-  if (momentum != 0.f) {
-    const float b = first_step ? g : momentum * mom[i] + g;
-    mom[i] = b;
-    g = b;
-  }
-  p -= lr * g;
-  master[i] = p;
-  if (param_bf16) param_bf16[i] = __float2bfloat16(p);
 }
 
 // bf16 -> fp32 accumulate / copy with scale: dst (+)= scale * src
@@ -745,15 +726,8 @@ __global__ void __launch_bounds__(256) adam_strided_kernel(float* __restrict__ m
   float pp[4] = {p.x, p.y, p.z, p.w}, mm[4] = {m.x, m.y, m.z, m.w}, vv[4] = {v.x, v.y, v.z, v.w};
   const float gg[4] = {g4.x, g4.y, g4.z, g4.w};
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    float g = gg[j] * grad_scale;
-    if (!adamw && weight_decay != 0.f) g += weight_decay * pp[j];
-    mm[j] = beta1 * mm[j] + (1.f - beta1) * g;
-    vv[j] = beta2 * vv[j] + (1.f - beta2) * g * g;
-    const float denom = sqrtf(vv[j] / bc2) + eps;
-    if (adamw && weight_decay != 0.f) pp[j] *= (1.f - lr * weight_decay);
-    pp[j] -= lr * (mm[j] / bc1) / denom;
-  }
+  for (int j = 0; j < 4; ++j)
+    adam_update(pp[j], mm[j], vv[j], gg[j], lr, beta1, beta2, eps, weight_decay, bc1, bc2, grad_scale, adamw);
   *reinterpret_cast<float4*>(master + i4) = make_float4(pp[0], pp[1], pp[2], pp[3]);
   *reinterpret_cast<float4*>(exp_avg + i4) = make_float4(mm[0], mm[1], mm[2], mm[3]);
   *reinterpret_cast<float4*>(exp_avg_sq + i4) = make_float4(vv[0], vv[1], vv[2], vv[3]);
@@ -771,17 +745,6 @@ extern "C" int pg_adam_strided(float* master, float* m, float* v, float* grad, v
                                                                        bucket_stride, total, lr, beta1, beta2, eps, wd, bc1,
                                                                        bc2, grad_scale, adamw, zero_grad);
   PG_CHECK_LAUNCH("adam_strided");
-  return 0;
-}
-
-extern "C" int pg_sgd(float* master, float* mom, const float* grad, void* param_bf16, int64_t n,
-                      float lr, float momentum, float wd, float grad_scale, int first_step,
-                      cudaStream_t s) {
-  if (n == 0) return 0;
-  sgd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(master, mom, grad,
-                                                         (__nv_bfloat16*)param_bf16, n, lr, momentum,
-                                                         wd, grad_scale, first_step);
-  PG_CHECK_LAUNCH("sgd");
   return 0;
 }
 

@@ -211,8 +211,6 @@ int pg_adam(float* master, float* m, float* v, const float* grad, void* param_bf
 int pg_adam_strided(float* master, float* m, float* v, float* grad, void* param_bf16, int64_t seg, int64_t bucket_stride,
                     int64_t nb, float lr, float beta1, float beta2, float eps, float wd, float bc1, float bc2,
                     float grad_scale, int adamw, int zero_grad, cudaStream_t s);
-int pg_sgd(float* master, float* mom, const float* grad, void* param_bf16, int64_t n, float lr,
-           float momentum, float wd, float grad_scale, int first_step, cudaStream_t s);
 int pg_accum_bf16_to_f32(const void* src, float* dst, int64_t n, float scale, int accumulate,
                          cudaStream_t s);
 

@@ -17,6 +17,22 @@ from pipegoose_b200.nn.tensor_parallel._utils import VocabUtility
 from pipegoose_b200.ops import kernels as K
 
 
+def _kernel_rows(logits2: torch.Tensor, copy: bool = False) -> torch.Tensor:
+    """``logits2`` laid out for the cross-entropy kernels, which read rows in 16-byte chunks: a leading dimension that
+    is a multiple of 8 elements.  A shard width that is not (GPT-2's 50257 at TP 2 gives 25129 per rank) is copied
+    into an 8-padded buffer and handed over as its ``[:, :v_local]`` view; the kernels never read the padding.
+    ``copy``: always return a new buffer of that layout (the backward kernel overwrites it in place)."""
+    from pipegoose_b200.ops import use_native
+
+    if not copy and (not use_native(logits2) or (logits2.stride(0) % 8 == 0 and logits2.data_ptr() % 16 == 0)):
+        return logits2
+    rows, v_local = logits2.shape
+    buf = torch.empty(rows, (v_local + 7) // 8 * 8, dtype=logits2.dtype, device=logits2.device)
+    view = buf[:, :v_local]
+    view.copy_(logits2)
+    return view
+
+
 class _VocabParallelCrossEntropy(torch.autograd.Function):
     @staticmethod
     def forward(ctx, parallel_logits: torch.Tensor, targets: torch.Tensor, parallel_context: ParallelContext):
@@ -27,6 +43,7 @@ class _VocabParallelCrossEntropy(torch.autograd.Function):
         logits2 = parallel_logits.reshape(-1, v_local)
         if not logits2.is_contiguous():
             logits2 = logits2.contiguous()
+        logits2 = _kernel_rows(logits2)
         tgt = targets.reshape(-1)
         stats = K.ce_local_stats(logits2, tgt, vocab_start)
         if world > 1:
@@ -49,7 +66,7 @@ class _VocabParallelCrossEntropy(torch.autograd.Function):
         if use_native(logits2) and g.numel() > 0 and (g.stride(0) == 0 or g.numel() == 1):
             # every token carries the same upstream gradient (``loss.mean()`` / ``loss.sum()``): one pass of the fused
             # kernel turns a bf16 copy of the logits into (softmax - onehot) * g — no fp32 [tokens, vocab/T] temporaries
-            work = logits2.clone()
+            work = _kernel_rows(logits2, copy=True)
             K.ce_finalize(work, tgt, gstats, ctx.vocab_start, g[:1].float().contiguous(), ignore_index=-(1 << 62), write_grad=True)
             return work.view(ctx.shape), None, None
         p = torch.exp(logits2.float() - gstats[:, 0:1]) / gstats[:, 1:2]
