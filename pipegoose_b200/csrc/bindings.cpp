@@ -27,7 +27,8 @@ void gemm(const torch::Tensor& a, const torch::Tensor& b, torch::Tensor out, boo
           const c10::optional<torch::Tensor>& aux, int64_t flags, int64_t block_n,
           int64_t max_ctas, int64_t num_chunks, int64_t first_chunk, int64_t chunk_flags_ptr,
           int64_t flag_value, std::vector<int64_t> out_peer_ptrs,
-          std::vector<int64_t> arrive_ctr_ptrs, const py::dict& ag) {
+          std::vector<int64_t> arrive_ctr_ptrs, const py::dict& ag,
+          const c10::optional<torch::Tensor>& bias_grad) {
   check_bf16_2d(a, "a");
   check_bf16_2d(b, "b");
   c10::cuda::CUDAGuard guard(a.device());
@@ -115,6 +116,14 @@ void gemm(const torch::Tensor& a, const torch::Tensor& b, torch::Tensor out, boo
   if (ag.contains("grad_rs")) {
     TORCH_CHECK(f32, "grad_rs needs an fp32 output");
     parse_grad_rs(ag["grad_rs"].cast<py::dict>(), &d.grad_rs);
+  }
+  if (bias_grad.has_value()) {
+    // wgrad with the bias gradient summed from the dY operand: bias_grad[m] += sum_k a[k, m]
+    TORCH_CHECK(a_mn && num_chunks == 1 && !ag.contains("n_comm"), "bias_grad needs a wgrad (a_mn) GEMM of one chunk");
+    TORCH_CHECK(bias_grad->is_cuda() && bias_grad->scalar_type() == torch::kFloat32 && bias_grad->is_contiguous() &&
+                    bias_grad->numel() == M, "bias_grad must be a contiguous fp32 CUDA tensor of ", M, " elements");
+    d.bias_grad = bias_grad->data_ptr<float>();
+    d.flags |= 256;
   }
   if (ag.contains("k_splits")) d.k_splits = ag["k_splits"].cast<int>();
   if (ag.contains("n_comm")) {
@@ -714,7 +723,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("flags") = 0, py::arg("block_n") = 0, py::arg("max_ctas") = 0,
         py::arg("num_chunks") = 1, py::arg("first_chunk") = 0, py::arg("chunk_flags_ptr") = 0,
         py::arg("flag_value") = 0, py::arg("out_peer_ptrs") = std::vector<int64_t>{},
-        py::arg("arrive_ctr_ptrs") = std::vector<int64_t>{}, py::arg("ag") = py::dict());
+        py::arg("arrive_ctr_ptrs") = std::vector<int64_t>{}, py::arg("ag") = py::dict(),
+        py::arg("bias_grad") = py::none());
   m.def("layernorm_fwd", &layernorm_fwd);
   m.def("layernorm_bwd", &layernorm_bwd);
   m.def("colsum", &colsum);

@@ -32,20 +32,20 @@ static PFN_encodeTiled get_encode_fn() {
   return fn;
 }
 
-// 2-D bf16 tensor map over a row-major [rows, cols] matrix (cols contiguous, leading
-// dimension ld elements) with a [box_rows, 64] box and 128-byte swizzle.
-int make_tmap_bf16_2d(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols,
-                      uint64_t ld, uint32_t box_rows, uint32_t box_cols) {
+// 2-D bf16 (fp32: f32 = true) tensor map over a row-major [rows, cols] matrix (cols contiguous, leading
+// dimension ld elements) with a [box_rows, box_cols] box and 128-byte swizzle.
+static int make_tmap_2d(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld,
+                        uint32_t box_rows, uint32_t box_cols, bool f32) {
   PFN_encodeTiled enc = get_encode_fn();
   if (!enc) return -1;
   // driver entry points need the primary context bound to the calling thread (autograd worker
   // threads have not necessarily touched the runtime yet)
   cudaFree(nullptr);
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * 2};
+  cuuint64_t strides[1] = {ld * (f32 ? 4 : 2)};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims,
+  CUresult r = enc(out, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims,
                    strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -58,6 +58,11 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t
     return -1;
   }
   return 0;
+}
+
+int make_tmap_bf16_2d(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols,
+                      uint64_t ld, uint32_t box_rows, uint32_t box_cols) {
+  return make_tmap_2d(out, ptr, rows, cols, ld, box_rows, box_cols, false);
 }
 
 // 3-D fp32 tensor map over a contiguous [d2, d1, d0] tensor (d0 contiguous) with a [1, box1, 32] box and 128-byte
@@ -85,8 +90,9 @@ struct TmapKey {
   const void* ptr;
   uint64_t rows, cols, ld;
   uint32_t box_rows;
+  bool f32;
   bool operator==(const TmapKey& o) const {
-    return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows;
+    return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && f32 == o.f32;
   }
 };
 struct TmapKeyHash {
@@ -94,23 +100,24 @@ struct TmapKeyHash {
     size_t h = reinterpret_cast<size_t>(k.ptr);
     h ^= k.rows * 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2);
     h ^= k.cols * 0xC2B2AE3D27D4EB4Full + (h << 6) + (h >> 2);
-    h ^= (k.ld * 31 + k.box_rows) + (h << 6) + (h >> 2);
+    h ^= (k.ld * 31 + k.box_rows * 2 + k.f32) + (h << 6) + (h >> 2);
     return h;
   }
 };
 
+// bf16 maps have [box_rows x 64] boxes, fp32 maps (f32 = true) [box_rows x 32]: 128-byte box rows either way
 static int cached_tmap(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols,
-                       uint64_t ld, uint32_t box_rows) {
+                       uint64_t ld, uint32_t box_rows, bool f32 = false) {
   static std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> cache;
   static std::mutex mu;
-  TmapKey key{ptr, rows, cols, ld, box_rows};
+  TmapKey key{ptr, rows, cols, ld, box_rows, f32};
   std::lock_guard<std::mutex> g(mu);
   auto it = cache.find(key);
   if (it != cache.end()) {
     *out = it->second;
     return 0;
   }
-  if (make_tmap_bf16_2d(out, ptr, rows, cols, ld, box_rows, 64) != 0) return -1;
+  if (make_tmap_2d(out, ptr, rows, cols, ld, box_rows, f32 ? 32 : 64, f32) != 0) return -1;
   if (cache.size() > 8192) cache.clear();
   cache.emplace(key, *out);
   return 0;
@@ -177,7 +184,8 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const CUtens
 
 // Tile width (and, for fp32-accumulating outputs, a K split) by a wave-quantisation cost model:
 // cost = waves * (k-blocks per work item * BN / efficiency(BN)) + one exposed epilogue.
-static int pick_bn(int M_rows, int N, int K, int chunks, int ctas, bool allow_split, int* k_splits) {
+// cheap_split: partial sums leave through the TMA epilogue's reduce-adds, which cost what a plain store costs.
+static int pick_bn(int M_rows, int N, int K, int chunks, int ctas, bool allow_split, bool cheap_split, int* k_splits) {
   const int cand[4] = {256, 192, 128, 64};
   const float eff[4] = {1.0f, 0.93f, 0.82f, 0.55f};  // 128 x BN tiles
   const int num_kb = (K + BK - 1) / BK;
@@ -193,8 +201,8 @@ static int pick_bn(int M_rows, int N, int K, int chunks, int ctas, bool allow_sp
       const int per = (num_kb + s - 1) / s;
       if (s > 1 && (per < 16 || (long)(s - 1) * per >= num_kb)) break;
       const long waves = (tiles * s + ctas - 1) / ctas;
-      // the epilogue of the last wave is exposed; atomics cost about twice a plain store
-      const float epi = (s > 1 ? 16.0f : 8.0f) * (float)bn;
+      // the epilogue of the last wave is exposed; per-thread atomics cost about twice a plain store
+      const float epi = (s > 1 && !cheap_split ? 16.0f : 8.0f) * (float)bn;
       const float cost = (float)waves * (float)per * (float)bn / eff[i] + epi;
       if (cost < best_cost * 0.97f) {
         best_cost = cost;
@@ -242,6 +250,12 @@ extern "C" int pg_gemm_bf16(const PgGemmDesc* d, cudaStream_t stream) {
   args.ce_part = d->ce_part;
   args.ce_valid = d->ce_valid > 0 ? d->ce_valid : d->N;
   args.grad_rs = d->grad_rs;
+  args.bias_grad = d->bias_grad;
+  if ((args.flags & EPI_BGRAD) &&
+      (!d->a_mn || args.bias_grad == nullptr || d->num_chunks > 1 || d->n_comm > 0)) {
+    fprintf(stderr, "pipegoose_b200: the fused bias gradient needs an MN-major A, a bias_grad buffer and one chunk\n");
+    return -1;
+  }
   if (args.grad_rs.world > 1) {
     if (!(d->flags & EPI_OUT_F32) || args.num_chunks > 1 || (d->ldc % 4) != 0) {
       fprintf(stderr, "pipegoose_b200: gradient reduce-scatter epilogue needs a plain fp32 output with ldc %% 4 == 0\n");
@@ -278,8 +292,14 @@ extern "C" int pg_gemm_bf16(const PgGemmDesc* d, cudaStream_t stream) {
   // split-K only where the epilogue can add partial sums: plain fp32 outputs (wgrad into main grads)
   const bool allow_split = (args.flags & EPI_OUT_F32) && args.num_chunks == 1 && args.bias == nullptr &&
                            d->k_splits != 1 && (d->ldc % 4) == 0;
+  // the TMA epilogue serves plain fp32 outputs (see tma_epi below)
+  const bool f32_tma = (args.flags & EPI_OUT_F32) && args.num_chunks == 1 && args.bias == nullptr &&
+                       (d->ldc % 4) == 0 && args.grad_rs.world <= 1 && args.n_comm == 0 && args.ce_part == nullptr &&
+                       !(args.flags & (EPI_GELU | EPI_RESIDUAL | EPI_DGELU | EPI_SCATTER)) &&
+                       (reinterpret_cast<uintptr_t>(args.out) & 15) == 0;
   int auto_splits = 1;
-  int bn = pick_bn(chunk_rows, args.N, args.K, args.num_chunks, max_ctas - args.n_comm, allow_split, &auto_splits);
+  int bn = pick_bn(chunk_rows, args.N, args.K, args.num_chunks, max_ctas - args.n_comm, allow_split, f32_tma,
+                   &auto_splits);
   if (args.ce_part != nullptr && d->block_n <= 0) {
     // the partials are laid out per 256-column tile (two per row and tile): fix the tile width
     bn = 256;
@@ -331,19 +351,25 @@ extern "C" int pg_gemm_bf16(const PgGemmDesc* d, cudaStream_t stream) {
 
   // The TMA-store epilogue serves every call with a bf16 output, one chunk (no fused collective, no MoE scatter)
   // and 16-byte-aligned matrices (TMA's requirement).  The GELU pre-activation output cannot share the slots with
-  // an epilogue input, so that combination also stays on the general epilogue.
+  // an epilogue input, so that combination also stays on the general epilogue.  It also serves plain fp32 outputs
+  // (f32_tma: no bias or other epilogue input, no gradient reduce-scatter), split or not: partial sums and
+  // accumulation leave as TMA reduce-adds.
   auto aligned = [](const void* p, int ld) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0 && (ld % 8) == 0; };
   const void* epi_in = (args.flags & EPI_DGELU) ? args.aux : (args.flags & EPI_RESIDUAL) ? args.residual : nullptr;
   const int in_ld = (args.flags & EPI_DGELU) ? args.ldc : args.ldr;
   const bool gelu_aux = (args.flags & EPI_GELU) && args.aux != nullptr;
-  const bool tma_epi = !(args.flags & (EPI_OUT_F32 | EPI_SCATTER)) && args.num_chunks == 1 && args.n_comm == 0 &&
-                       args.grad_rs.world <= 1 && args.k_splits == 1 && aligned(args.out, args.ldc) &&
-                       (!gelu_aux || (aligned(args.aux, args.ldc) && epi_in == nullptr)) &&
-                       (epi_in == nullptr || aligned(epi_in, in_ld)) &&
-                       (!(args.flags & EPI_BIAS) || aligned(args.bias, 8));
+  const bool tma_epi = f32_tma || (!(args.flags & (EPI_OUT_F32 | EPI_SCATTER)) && args.num_chunks == 1 &&
+                                   args.n_comm == 0 && args.grad_rs.world <= 1 && args.k_splits == 1 &&
+                                   aligned(args.out, args.ldc) &&
+                                   (!gelu_aux || (aligned(args.aux, args.ldc) && epi_in == nullptr)) &&
+                                   (epi_in == nullptr || aligned(epi_in, in_ld)) &&
+                                   (!(args.flags & EPI_BIAS) || aligned(args.bias, 8)));
   EpiMaps em;
   memset(&em, 0, sizeof(em));
-  if (tma_epi) {
+  if (f32_tma) {
+    if (cached_tmap(&em.out, args.out, args.M, args.N, args.ldc, 64, true) != 0) return -1;
+    em.aux = em.in = em.out;
+  } else if (tma_epi) {
     if (cached_tmap(&em.out, args.out, args.M, args.N, args.ldc, 64) != 0) return -1;
     em.aux = em.in = em.out;
     if (gelu_aux && cached_tmap(&em.aux, args.aux, args.M, args.N, args.ldc, 64) != 0) return -1;

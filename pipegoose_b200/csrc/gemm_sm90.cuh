@@ -1,8 +1,9 @@
 // Persistent, warp-specialised bf16 GEMM for sm_90a:
 //   TMA (cp.async.bulk.tensor) -> 128B-swizzled smem ring -> wgmma.mma_async issued by two
 //   consumer warpgroups (64 rows of the 128-row tile each, fp32 accumulators in registers) ->
-//   epilogue by the same warpgroups: for bf16 outputs in the accumulator-fragment layout with TMA stores
-//   (epilogue_tma), otherwise accumulators handed over through shared memory (the general epilogue).
+//   epilogue by the same warpgroups: for bf16 and plain fp32 outputs in the accumulator-fragment layout with TMA
+//   stores / reduce-adds (epilogue_tma, epilogue_tma_f32), otherwise accumulators handed over through shared memory
+//   (the general epilogue).
 //
 // One kernel serves the three operand layouts a transformer training step needs
 //   NT : Y  = X  · Wᵀ   (A K-major,  B K-major)    forward
@@ -36,6 +37,7 @@ enum EpiFlags : int {
   EPI_DGELU = 32,      // out = acc * gelu_tanh'(aux_in[row, col])
   EPI_SCATTER = 64,    // MoE combine: out row -> out_peer[src][row_ret[row]], scaled by row_scale[row]
   EPI_ATOMIC = 128,    // fp32 out += acc with red.global.add (split-K partial sums)
+  EPI_BGRAD = 256,     // bias_grad[m] += sum_k A[k, m] (wgrad: the bias gradient from the dY operand, A MN-major)
 };
 // (GemmArgs::ce_part != null) lm_head: besides the bf16 logits the epilogue emits, per row and per half tile, the online
 // softmax partials (max, sum exp(x - max)) of the logits it holds in registers — the cross entropy never re-reads the
@@ -43,7 +45,7 @@ enum EpiFlags : int {
 
 struct GemmArgs {
   int M, N, K;
-  int k_splits;  // >1: the K loop is split over k_splits work items per tile (EPI_ATOMIC epilogue)
+  int k_splits;  // >1: the K loop is split over k_splits work items per tile (partial sums added: EPI_ATOMIC)
   void* out;
   int ldc;
   const __nv_bfloat16* bias;
@@ -93,6 +95,7 @@ struct GemmArgs {
   // wgrad -> data-parallel reduce-scatter (fp32 outputs): every 16-byte group of the tile is added into the gradient
   // buffer of the rank that owns its ZeRO-1 slice (local L2 atomics / NVLink peer atomics); grad_rs.world <= 1: off
   PgGradRS grad_rs;
+  float* bias_grad;  // EPI_BGRAD: fp32 [M]
 };
 
 constexpr int BM = 128;
@@ -305,6 +308,59 @@ PG_DEVICE void epilogue_tma(float (&acc)[BN / 2], const GemmArgs& args, const CU
   store_tile(tma_out);
 }
 
+// TMA epilogue of one tile for consumer warpgroup wg, plain fp32 output (wgrad into a main grad).  The warpgroup's
+// BN / 64 slots of 8 KB hold [64 rows x 32] fp32 each (one 128-byte row per tile row, 128B-swizzled), so its
+// 64 x BN block leaves in two rounds of BN / 2 columns; the second round reuses the slots once the first round's
+// transfers have read them.  With EPI_ACCUM (accumulate, or a split-K partial) the slots are added to the output
+// with TMA reduce-adds, else stored.  Both are clipped at the M / N edges.
+//
+// Fragment pair acc[4 j + 2 hh + (0, 1)] (row r = 16 wl + lane / 4 + 8 hh, columns 8 j + 2 quad + (0, 1)) is 8 bytes
+// of 16-byte chunk 2 (j % 4) + quad / 2 of row r in slot (j % (BN / 16)) / 4 of round j / (BN / 16), stored at chunk
+// position chunk ^ (r % 8): a warp's 256 bytes cover every bank twice (the minimum for 8-byte stores).
+template <int BN>
+PG_DEVICE void epilogue_tma_f32(const float (&acc)[BN / 2], const GemmArgs& args, const CUtensorMap* tma_out,
+                                uint8_t* wslots, int m_blk, int n_blk, int wg, int tid_wg) {
+  constexpr int kSlotBytes = 64 * 32 * 4;
+  constexpr int JR = BN / 16;  // fragment column groups per round
+  const int lane = tid_wg & 31;
+  const int wl = tid_wg >> 5;
+  const int quad = lane & 3;
+  const int m0 = m_blk * BM + 64 * wg;
+  const int n0 = n_blk * BN;
+  const bool add = (args.flags & EPI_ACCUM) != 0;
+  uint8_t* my_row = wslots + (16 * wl + (lane >> 2)) * 128 + (quad & 1) * 8;
+  named_bar_sync(2 + wg, 128);  // the storing thread saw the previous tile's transfers read the slots
+#pragma unroll
+  for (int rd = 0; rd < 2; ++rd) {
+    if (rd == 1) {
+      if (tid_wg == 0) tma_store_wait_read<0>();
+      named_bar_sync(2 + wg, 128);
+    }
+#pragma unroll
+    for (int jj = 0; jj < JR; ++jj) {
+      const int j = rd * JR + jj;
+      const int chunk = 2 * (jj & 3) + (quad >> 1);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+        *reinterpret_cast<float2*>(my_row + (jj >> 2) * kSlotBytes + hh * (8 * 128) + ((chunk ^ (lane >> 2)) << 4)) =
+            make_float2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]);
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(2 + wg, 128);
+    if (tid_wg == 0) {
+#pragma unroll
+      for (int s = 0; s < BN / 64; ++s) {
+        const int c0 = n0 + rd * (BN / 2) + 32 * s;
+        if (add)
+          tma_reduce_add_2d(tma_out, wslots + s * kSlotBytes, c0, m0);
+        else
+          tma_store_2d(tma_out, wslots + s * kSlotBytes, c0, m0);
+      }
+      tma_store_commit();
+    }
+  }
+}
+
 // Register budget: the block owns the SM's register file (384 threads x 168 at launch); the producer warpgroup gives
 // registers back (40) and the two consumer warpgroups take them (232): 128*40 + 256*232 <= 64 K.  A consumer thread
 // holds BN/2 fp32 accumulators (128 at BN = 256) plus the epilogue's working set.
@@ -341,6 +397,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
   uint64_t* epi_empty = bars + 2 * STAGES + 1;  // TMA_EPI: both warpgroups' previous stores have read the slots
   // TMA_EPI: the producer warpgroup prefetches epilogue operands (uniform over the grid)
   const bool has_in = TMA_EPI && ((args.flags & EPI_BIAS) || epi_input(args) != nullptr);
+  // warps 2, 3 sum the A stages into the bias gradient (uniform over the grid; wgrad layout only)
+  const bool bgrad = A_MN && (args.flags & EPI_BGRAD) != 0;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -435,7 +493,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 2);  // one arrival per consumer warpgroup
+      mbar_init(&empty_bar[i], bgrad ? 4 : 2);  // one arrival per consumer warpgroup (+ warps 2, 3: EPI_BGRAD)
     }
     if constexpr (TMA_EPI) {
       mbar_init(epi_full, 1);
@@ -526,6 +584,48 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
       __syncwarp();
       parity ^= 1;
     }
+  } else if (A_MN && bgrad && (warp == 2 || warp == 3)) {
+    // ============================ bias gradient (EPI_BGRAD) ============================
+    // bias_grad[m] = sum over k of A[k, m], read from the stages the main loop consumes: warp 2 + i sums the
+    // [64 k x 64 m] box i of every stage it owns, lane l columns 2 l, 2 l + 1 (16-byte chunk l / 4 of a 128-byte
+    // row, at chunk (l / 4) ^ (k % 8)).  Every tile of an M block streams the same A, so a tile sums only the
+    // k-blocks with kb % n_blks == n_blk: each k-block is read once per M block, whatever the split.  The warp
+    // releases each stage with its own arrival on the empty barrier and adds its sums once per work item.
+    const int i = warp - 2;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int t = unit0; t < num_work; t += unit_stride) {
+      const TileCoord tc = map_tile(t % num_tiles, m_blks_per_chunk, n_blks, args.num_chunks, args.first_chunk);
+      const int kb_begin = (t / num_tiles) * kb_per_split;
+      const int kb_end = min(num_kb, kb_begin + kb_per_split);
+      float s0 = 0.f, s1 = 0.f;
+      bool summed = false;
+      for (int kb = kb_begin; kb < kb_end; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        if (kb % n_blks == tc.n_blk) {
+          const uint8_t* box = smem_a + stage * Cfg::kABytes + i * (BK * 128) + (lane & 3) * 4;
+#pragma unroll 8
+          for (int k = 0; k < BK; ++k) {
+            const float2 v =
+                unpack_bf16x2(*reinterpret_cast<const uint32_t*>(box + k * 128 + (((lane >> 2) ^ (k & 7)) << 4)));
+            s0 += v.x;
+            s1 += v.y;
+          }
+          summed = true;
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      const int m = tc.m_blk * BM + 64 * i + 2 * lane;
+      if (summed && m < args.M) {
+        atomicAdd(args.bias_grad + m, s0);
+        if (m + 1 < args.M) atomicAdd(args.bias_grad + m + 1, s1);
+      }
+    }
   }
   } else {
     setmaxnreg_inc<kGemmConsumerRegs>();
@@ -611,8 +711,13 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         if (prev_stage >= 0 && tid_wg == 0) mbar_arrive(&empty_bar[prev_stage]);
       }
       if constexpr (TMA_EPI) {
-        epilogue_tma<BN>(acc, args, &tma_out, &tma_aux, smem_slots + wg * (BN / 64) * Cfg::kSlotBytes, smem_bias,
-                         epi_full, epi_parity, has_in, tc.m_blk, tc.n_blk, n_blks, wg, tid_wg);
+        uint8_t* wslots = smem_slots + wg * (BN / 64) * Cfg::kSlotBytes;
+        if (out_f32) {
+          epilogue_tma_f32<BN>(acc, args, &tma_out, wslots, tc.m_blk, tc.n_blk, wg, tid_wg);
+          continue;
+        }
+        epilogue_tma<BN>(acc, args, &tma_out, &tma_aux, wslots, smem_bias, epi_full, epi_parity, has_in, tc.m_blk,
+                         tc.n_blk, n_blks, wg, tid_wg);
         epi_parity ^= 1;
         continue;
       }

@@ -71,6 +71,9 @@ typedef struct PgGemmDesc {
   // columns >= ce_valid are padding.  block_n is forced to 256 so that the caller can size the buffer.
   float* ce_part;
   int ce_valid;
+  // wgrad (a_mn): with EPI_BGRAD (256) in flags, bias_grad[m] (fp32 [M]) += sum over k of A[k, m], the bias gradient
+  // summed from the dY stages the GEMM already loads
+  float* bias_grad;
 } PgGemmDesc;
 
 // ---- attention_sm90.cu

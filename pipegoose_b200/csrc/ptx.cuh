@@ -114,6 +114,13 @@ PG_DEVICE void tma_reduce_add_3d(const CUtensorMap* m, const void* smem_src, int
       "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+PG_DEVICE void tma_reduce_add_2d(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1) {
+  asm volatile(
+      "cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
+          reinterpret_cast<uint64_t>(m)),
+      "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+      : "memory");
+}
 PG_DEVICE void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 PG_DEVICE void tma_store_wait_read() {

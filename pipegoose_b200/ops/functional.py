@@ -81,6 +81,19 @@ def _bgrad(dy, bias):
     return K.colsum(dy).to(bias.dtype)
 
 
+def _wgrad_bgrad(dy, x, weight, bias):
+    """``(_wgrad(dy, x, weight), _bgrad(dy, bias))``.  When both parameters have main grads, one GEMM computes both:
+    the wgrad sums the bias gradient from the ``dy`` tiles it already loads, so ``dy`` is read once."""
+    if bias is None or _main_grad(weight) is None or _main_grad(bias) is None:
+        return _wgrad(dy, x, weight), _bgrad(dy, bias)
+    mg, accumulate = acquire_main_grad(weight, will_overwrite=True)
+    mg_b, _ = acquire_main_grad(bias, will_overwrite=False)
+    K.gemm_tn(dy, x, accum_into=mg, accumulate=accumulate, bias_grad=mg_b)
+    notify_grad_ready(weight)
+    notify_grad_ready(bias)
+    return None, None
+
+
 def _ln_bwd(dy, x, gamma, beta, mean, rstd, dx_extra=None, tp=None):
     # Under fused TP the dx of a sub-layer is the dy of the one before it, whose first backward op is an
     # all-gather->GEMM: writing dx straight into that all-gather's staging slot saves a 16 MB copy per sub-layer.
@@ -115,8 +128,7 @@ def _ln_linear_bwd(dy, x, gamma, beta, weight, bias, mean, rstd, ln_full, tp, dx
     else:
         dln_full = K.gemm_nn(dy, weight)
         dln = tp.reduce_scatter_rows(dln_full) if tp is not None else dln_full
-    dw = _wgrad(dy, ln_full, weight)
-    db = _bgrad(dy, bias)
+    dw, db = _wgrad_bgrad(dy, ln_full, weight, bias)
     dx, dgamma, dbeta = _ln_bwd(dln, x, gamma, beta, mean, rstd, dx_extra=dx_extra, tp=tp)
     return dx, dgamma, dbeta, dw, db
 
@@ -139,6 +151,9 @@ def _linear_residual_bwd(dy, a, weight, bias, tp):
     else:
         dy_full = tp.all_gather_rows(dy)
         da = K.gemm_nn(dy_full, weight)
+    if tp is None:
+        dw, db = _wgrad_bgrad(dy, a, weight, bias)
+        return da, dw, db
     dw = _wgrad(dy_full, a, weight)
     # the bias is replicated across TP ranks: each rank sums its own token shard and the
     # gradient reducer adds the TP group's partial sums (see DataParallel / grad buffer).
@@ -266,15 +281,18 @@ class LayerNormMLP(torch.autograd.Function):
         else:
             dy_full = tp.all_gather_rows(dy)
             dz = K.gemm_nn(dy_full, w2, dgelu_aux=z)
-        dw2 = _wgrad(dy_full, h1, w2)
-        db2 = _bgrad(dy, b2)
+        if tp is None:
+            dw2, db2 = _wgrad_bgrad(dy, h1, w2, b2)
+        else:
+            # row-parallel: the wgrad reads every rank's tokens, the bias sums this rank's shard (see above)
+            dw2 = _wgrad(dy_full, h1, w2)
+            db2 = _bgrad(dy, b2)
         if tp is not None and tp.fused:
             dln = tp.gemm_rs_nn(dz, w1)
         else:
             dln_full = K.gemm_nn(dz, w1)
             dln = tp.reduce_scatter_rows(dln_full) if tp is not None else dln_full
-        dw1 = _wgrad(dz, ln_full, w1)
-        db1 = _bgrad(dz, b1)
+        dw1, db1 = _wgrad_bgrad(dz, ln_full, w1, b1)
         # residual gradient (dy) is added inside the LN backward kernel
         dx, dgamma, dbeta = _ln_bwd(dln, x, gamma, beta, mean, rstd, dx_extra=dy, tp=tp)
         return dx, dgamma, dbeta, dw1, db1, dw2, db2, None, None

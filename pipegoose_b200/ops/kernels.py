@@ -103,9 +103,12 @@ def gemm_nn(dy, w, dgelu_aux=None, out=None, **kw):
     return y
 
 
-def gemm_tn(dy, x, accum_into: Optional[torch.Tensor] = None, accumulate: bool = True, **kw):
+def gemm_tn(dy, x, accum_into: Optional[torch.Tensor] = None, accumulate: bool = True,
+            bias_grad: Optional[torch.Tensor] = None, **kw):
     """``dW[N,K] = dy[M,N]^T @ x[M,K]`` (wgrad).  With ``accum_into`` (fp32 main grad) the product is
-    accumulated in place by the GEMM epilogue and ``None`` is returned."""
+    accumulated in place by the GEMM epilogue and ``None`` is returned.  ``bias_grad`` (fp32 ``[N]``, with
+    ``accum_into``): the column sums of ``dy`` are added into it by the same kernel (``colsum(dy, bias_grad)``)."""
+    assert bias_grad is None or accum_into is not None, "bias_grad needs accum_into"
     if use_native(dy, x):
         N, K = dy.shape[1], x.shape[1]
         if accum_into is not None:
@@ -116,11 +119,13 @@ def gemm_tn(dy, x, accum_into: Optional[torch.Tensor] = None, accumulate: bool =
                 kw["ag"] = dict(kw.get("ag") or {}, grad_rs=rs)
                 accumulate = True
             native().gemm(dy, x, accum_into.view(N, K), True, True, None, None, None,
-                          EPI_ACCUM if accumulate else 0, **kw)
+                          EPI_ACCUM if accumulate else 0, bias_grad=bias_grad, **kw)
             return None
         out = torch.empty(N, K, dtype=torch.bfloat16, device=dy.device)
         native().gemm(dy, x, out, True, True, None, None, None, 0, **kw)
         return out
+    if bias_grad is not None:
+        colsum(dy, accum_into=bias_grad)
     g = dy.t() @ x
     if accum_into is not None:
         if accumulate:

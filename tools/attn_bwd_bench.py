@@ -35,7 +35,10 @@ def _kernel_times(prof, n_calls):
         us = getattr(e, "self_device_time_total", None)
         if us is None:
             us = e.self_cuda_time_total
-        out[e.key.split("(")[0].split("<")[0].strip()] = (e.count / n_calls, us / n_calls)
+        # template instantiations of one kernel share the name: add them up
+        name = e.key.split("(")[0].split("<")[0].strip()
+        c0, us0 = out.get(name, (0.0, 0.0))
+        out[name] = (c0 + e.count / n_calls, us0 + us / n_calls)
     return out
 
 

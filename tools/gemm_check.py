@@ -122,6 +122,11 @@ def epi_perf():
     ov = torch.empty(M, V, device=dev, dtype=torch.bfloat16)
     ce_part = torch.empty(M, 2 * ((V + 255) // 256), 2, device=dev, dtype=torch.float32)
     ce_ag = {"ce_part": ce_part.data_ptr(), "ce_valid": V}
+    # wgrad operands: dy of qkv [M, 3h]; fp32 main grads of fc2 [h, 4h], qkv [3h, h] and the lm_head table [V, h]
+    x3 = torch.randn(M, 3 * h, device=dev, dtype=torch.bfloat16)
+    g14 = torch.zeros(h, 4 * h, device=dev, dtype=torch.float32)
+    g3 = torch.zeros(3 * h, h, device=dev, dtype=torch.float32)
+    gv = torch.zeros(V, h, device=dev, dtype=torch.float32)
     cases = {
         "fc1_bias_gelu_aux": (lambda: _C.gemm(x, w1, o4, False, False, b4, None, z4, 2), 2.0 * M * h * 4 * h),
         "fc1_bias_only": (lambda: _C.gemm(x, w1, o4, False, False, b4, None, None, 0), 2.0 * M * h * 4 * h),
@@ -135,7 +140,30 @@ def epi_perf():
         "dense_wgrad_f32acc": (lambda: _C.gemm(x, x, g1, True, True, None, None, None, 16), 2.0 * M * h * h),
         "dense_wgrad_f32over": (lambda: _C.gemm(x, x, g1, True, True, None, None, None, 0), 2.0 * M * h * h),
         "fc1_wgrad_f32acc": (lambda: _C.gemm(x4, x, g4, True, True, None, None, None, 16), 2.0 * M * h * 4 * h),
+        "fc2_wgrad_f32acc": (lambda: _C.gemm(x, x4, g14, True, True, None, None, None, 16), 2.0 * M * h * 4 * h),
+        "qkv_wgrad_f32acc": (lambda: _C.gemm(x3, x, g3, True, True, None, None, None, 16), 2.0 * M * h * 3 * h),
+        "lm_head_wgrad_f32over": (lambda: _C.gemm(ov, x, gv, True, True, None, None, None, 0), 2.0 * M * h * V),
     }
+    # "+ bias sum": the wgrad that also produces the bias gradient (dy's column sums); a build without the fused form
+    # (no bias_grad argument) runs the wgrad and then the column-sum kernel, as its training step does
+    bg = torch.zeros(V, device=dev, dtype=torch.float32)
+    try:
+        _C.gemm(x, x, g1, True, True, None, None, None, 16, bias_grad=bg[:h])
+        fused = True
+    except TypeError:
+        fused = False
+
+    def with_bias(dy, xx, g, flags):
+        if fused:
+            return lambda: _C.gemm(dy, xx, g, True, True, None, None, None, flags, bias_grad=bg[:dy.shape[1]])
+        return lambda: (_C.gemm(dy, xx, g, True, True, None, None, None, flags), _C.colsum(dy, bg[:dy.shape[1]]))
+
+    for name, (dy, xx, g, flags, fl) in {"dense_wgrad_f32acc": (x, x, g1, 16, 2.0 * M * h * h),
+                                         "fc1_wgrad_f32acc": (x4, x, g4, 16, 2.0 * M * h * 4 * h),
+                                         "fc2_wgrad_f32acc": (x, x4, g14, 16, 2.0 * M * h * 4 * h),
+                                         "qkv_wgrad_f32acc": (x3, x, g3, 16, 2.0 * M * h * 3 * h),
+                                         "lm_head_wgrad_f32over": (ov, x, gv, 0, 2.0 * M * h * V)}.items():
+        cases[name + "_bias"] = (with_bias(dy, xx, g, flags), fl)
     out = {}
     for name, (fn, fl) in cases.items():
         row = {}
@@ -143,7 +171,7 @@ def epi_perf():
         row["auto"] = dict(ms=med, tflops=fl / med / 1e9)
         out[name] = row
         print(name, "  ".join(f"{t}: {v['ms']*1e3:.1f} us {v['tflops']:.0f} TF" for t, v in row.items()), flush=True)
-    del wv, ov, ce_part
+    del wv, ov, ce_part, gv
     return out
 
 # Plain NT GEMM at M = 8192, N = 4096, BN = 256 over K: time per tile round = fixed + per_kb * (K / 64).  The fit
