@@ -143,6 +143,125 @@ void gemm(const torch::Tensor& a, const torch::Tensor& b, torch::Tensor out, boo
 }
 
 
+bool is_fp8(const torch::Tensor& t) {
+  return t.scalar_type() == torch::kFloat8_e4m3fn || t.scalar_type() == torch::kFloat8_e5m2;
+}
+
+// out[M, N] = epilogue(a_scale_inv * b_scale_inv * (a[M, K] · b[N, K]ᵀ)) over FP8 codes, both K-major: a e4m3 or e5m2,
+// b e4m3.  bf16 out: bias, gelu (pre-activation into aux), residual, or dgelu (out *= gelu'(aux)); fp32 out: overwrite
+// or accumulate, k_splits 0 = auto, 1 = never, > 1 = forced.
+void gemm_fp8(const torch::Tensor& a, const torch::Tensor& b, const torch::Tensor& a_scale_inv,
+              const torch::Tensor& b_scale_inv, torch::Tensor out, const c10::optional<torch::Tensor>& bias,
+              const c10::optional<torch::Tensor>& residual, const c10::optional<torch::Tensor>& aux, bool gelu,
+              bool dgelu, bool accumulate, int64_t block_n, int64_t k_splits) {
+  for (const torch::Tensor* t : {&a, &b}) {
+    TORCH_CHECK(t->is_cuda() && t->device() == a.device(), "gemm_fp8: operands must be CUDA tensors on one device");
+    TORCH_CHECK(t->dim() == 2 && t->stride(1) == 1, "gemm_fp8: operands must be 2-D with unit inner stride");
+    TORCH_CHECK(t->stride(0) % 16 == 0 && reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0,
+                "gemm_fp8: operand rows must be 16-byte aligned (leading dimension a multiple of 16)");
+  }
+  TORCH_CHECK(is_fp8(a), "gemm_fp8: a must be float8_e4m3fn or float8_e5m2");
+  TORCH_CHECK(b.scalar_type() == torch::kFloat8_e4m3fn, "gemm_fp8: b must be float8_e4m3fn");
+  const int64_t M = a.size(0), K = a.size(1), N = b.size(0);
+  TORCH_CHECK(b.size(1) == K, "gemm_fp8: contraction dims differ: ", K, " vs ", b.size(1));
+  TORCH_CHECK(K % 16 == 0, "gemm_fp8: K (", K, ") must be a multiple of 16");
+  TORCH_CHECK(N % 8 == 0, "gemm_fp8: N must be a multiple of 8");
+  for (const torch::Tensor* t : {&a_scale_inv, &b_scale_inv})
+    TORCH_CHECK(t->is_cuda() && t->device() == a.device() && t->scalar_type() == torch::kFloat32 && t->numel() >= 1,
+                "gemm_fp8: scale_inv must be an fp32 CUDA scalar");
+  c10::cuda::CUDAGuard guard(a.device());
+  TORCH_CHECK(out.is_cuda() && out.dim() == 2 && out.stride(1) == 1 && out.size(0) == M && out.size(1) == N,
+              "gemm_fp8: out must be a 2-D CUDA tensor [M, N] with unit inner stride");
+  const bool f32 = out.scalar_type() == torch::kFloat32;
+  TORCH_CHECK(f32 || out.scalar_type() == torch::kBFloat16, "gemm_fp8: out must be bf16 or fp32");
+  TORCH_CHECK(out.stride(0) % 8 == 0 && reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0,
+              "gemm_fp8: out must be 16-byte aligned with a leading dimension that is a multiple of 8");
+  TORCH_CHECK(!f32 || (!bias.has_value() && !residual.has_value() && !aux.has_value() && !gelu && !dgelu),
+              "gemm_fp8: an fp32 out takes no epilogue input");
+  TORCH_CHECK(f32 || (!accumulate && k_splits <= 1), "gemm_fp8: accumulate / k_splits need an fp32 out");
+  TORCH_CHECK(!(gelu && dgelu) && !(dgelu && residual.has_value()), "gemm_fp8: gelu, dgelu and residual conflict");
+  TORCH_CHECK((gelu || dgelu) || !aux.has_value(), "gemm_fp8: aux is the GELU pre-activation (gelu / dgelu)");
+  TORCH_CHECK(!dgelu || aux.has_value(), "gemm_fp8: dgelu needs aux");
+  TORCH_CHECK(block_n == 0 || block_n == 64 || block_n == 128, "gemm_fp8: block_n must be 0 (auto), 64 or 128");
+  PgGemmDesc d;
+  memset(&d, 0, sizeof(d));
+  d.A = a.data_ptr();
+  d.B = b.data_ptr();
+  d.M = (int)M; d.N = (int)N; d.K = (int)K;
+  d.lda = (int)a.stride(0);
+  d.ldb = (int)b.stride(0);
+  d.out = out.data_ptr();
+  d.ldc = (int)out.stride(0);
+  d.flags = (f32 ? 8 : 0) | (gelu ? 2 : 0) | (dgelu ? 32 : 0) | (accumulate ? 16 : 0);
+  if (bias.has_value()) {
+    TORCH_CHECK(bias->is_cuda() && bias->scalar_type() == torch::kBFloat16 && bias->numel() == N && bias->is_contiguous(),
+                "gemm_fp8: bias must be contiguous bf16 [N]");
+    d.bias = bias->data_ptr();
+    d.flags |= 1;
+  }
+  if (residual.has_value()) {
+    check_bf16_2d(*residual, "residual");
+    TORCH_CHECK(residual->size(0) == M && residual->size(1) == N, "gemm_fp8: residual must be [M, N]");
+    d.residual = residual->data_ptr();
+    d.ldr = (int)residual->stride(0);
+    d.flags |= 4;
+  }
+  if (aux.has_value()) {
+    check_bf16_2d(*aux, "aux");
+    TORCH_CHECK(aux->size(0) == M && aux->size(1) == N && aux->stride(0) == out.stride(0), "gemm_fp8: aux must match out");
+    d.aux = aux->data_ptr();
+  }
+  d.block_n = (int)block_n;
+  d.k_splits = (int)k_splits;
+  d.num_chunks = 1;
+  d.fmt = a.scalar_type() == torch::kFloat8_e5m2 ? 2 : 1;
+  d.a_scale_inv = a_scale_inv.data_ptr<float>();
+  d.b_scale_inv = b_scale_inv.data_ptr<float>();
+  TORCH_CHECK(pg_gemm_bf16(&d, cur_stream()) == 0, "gemm_fp8 failed");
+}
+
+// Per-tensor FP8 cast of x bf16 [R, C] (contiguous, C % 8 == 0): amax (fp32 workspace, >= 1 element) = max |x|, then
+// each given output: codes [R, C] and codes_t [C, R] (float8_e5m2 when e5m2, else float8_e4m3fn), scale_inv (fp32
+// scalar) and colsum (fp32 [C], the column sums of x added into it).  Format: csrc/fp8_cast.cu.
+void fp8_quantize(const torch::Tensor& x, bool e5m2, torch::Tensor amax, const c10::optional<torch::Tensor>& codes,
+                  const c10::optional<torch::Tensor>& codes_t, const c10::optional<torch::Tensor>& scale_inv,
+                  const c10::optional<torch::Tensor>& colsum) {
+  TORCH_CHECK(x.is_cuda() && x.is_contiguous() && x.dim() == 2 && x.scalar_type() == torch::kBFloat16,
+              "fp8_quantize: x must be a contiguous 2-D bf16 CUDA tensor");
+  const int64_t R = x.size(0), C = x.size(1);
+  TORCH_CHECK(C % 8 == 0, "fp8_quantize: the column count (", C, ") must be a multiple of 8");
+  TORCH_CHECK(R < (int64_t(1) << 31) && C < (int64_t(1) << 31), "fp8_quantize: x is too large");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0, "fp8_quantize: x must be 16-byte aligned");
+  c10::cuda::CUDAGuard guard(x.device());
+  auto on_dev = [&](const torch::Tensor& t) { return t.is_cuda() && t.device() == x.device() && t.is_contiguous(); };
+  TORCH_CHECK(on_dev(amax) && amax.scalar_type() == torch::kFloat32 && amax.numel() >= 1,
+              "fp8_quantize: amax must be an fp32 CUDA workspace on x's device");
+  const auto dt = e5m2 ? torch::kFloat8_e5m2 : torch::kFloat8_e4m3fn;
+  if (codes.has_value())
+    TORCH_CHECK(on_dev(*codes) && codes->scalar_type() == dt && codes->size(0) == R && codes->size(1) == C &&
+                    reinterpret_cast<uintptr_t>(codes->data_ptr()) % 8 == 0,
+                "fp8_quantize: codes must be a contiguous 8-byte-aligned ", e5m2 ? "float8_e5m2" : "float8_e4m3fn",
+                " tensor [R, C]");
+  if (codes_t.has_value())
+    TORCH_CHECK(on_dev(*codes_t) && codes_t->scalar_type() == dt && codes_t->size(0) == C && codes_t->size(1) == R &&
+                    reinterpret_cast<uintptr_t>(codes_t->data_ptr()) % 16 == 0,
+                "fp8_quantize: codes_t must be a contiguous 16-byte-aligned ", e5m2 ? "float8_e5m2" : "float8_e4m3fn",
+                " tensor [C, R]");
+  if (scale_inv.has_value())
+    TORCH_CHECK(on_dev(*scale_inv) && scale_inv->scalar_type() == torch::kFloat32 && scale_inv->numel() >= 1,
+                "fp8_quantize: scale_inv must be an fp32 CUDA scalar");
+  if (colsum.has_value())
+    TORCH_CHECK(on_dev(*colsum) && colsum->scalar_type() == torch::kFloat32 && colsum->numel() == C,
+                "fp8_quantize: colsum must be a contiguous fp32 CUDA tensor of ", C, " elements");
+  TORCH_CHECK(pg_fp8_amax(x.data_ptr(), x.numel(), amax.data_ptr<float>(), cur_stream()) == 0, "fp8_amax failed");
+  TORCH_CHECK(pg_fp8_cast(x.data_ptr(), (int)R, (int)C, e5m2 ? 1 : 0, amax.data_ptr<float>(),
+                          codes.has_value() ? codes->data_ptr() : nullptr,
+                          codes_t.has_value() ? codes_t->data_ptr() : nullptr,
+                          scale_inv.has_value() ? scale_inv->data_ptr<float>() : nullptr,
+                          colsum.has_value() ? colsum->data_ptr<float>() : nullptr, cur_stream()) == 0,
+              "fp8_cast failed");
+}
+
 // {"peer": [ptr per data-parallel rank], "local": ptr, "start": elems, "seg": elems, "scalar": 0/1} -> PgGradRS
 bool parse_grad_rs(const py::dict& d, PgGradRS* out) {
   memset(out, 0, sizeof(*out));
@@ -725,6 +844,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("flag_value") = 0, py::arg("out_peer_ptrs") = std::vector<int64_t>{},
         py::arg("arrive_ctr_ptrs") = std::vector<int64_t>{}, py::arg("ag") = py::dict(),
         py::arg("bias_grad") = py::none());
+  m.def("gemm_fp8", &gemm_fp8, "wgmma FP8 GEMM (K-major e4m3 / e5m2 x e4m3 codes, per-tensor scales)", py::arg("a"),
+        py::arg("b"), py::arg("a_scale_inv"), py::arg("b_scale_inv"), py::arg("out"), py::arg("bias") = py::none(),
+        py::arg("residual") = py::none(), py::arg("aux") = py::none(), py::arg("gelu") = false, py::arg("dgelu") = false,
+        py::arg("accumulate") = false, py::arg("block_n") = 0, py::arg("k_splits") = 0);
+  m.def("fp8_quantize", &fp8_quantize, py::arg("x"), py::arg("e5m2"), py::arg("amax"), py::arg("codes") = py::none(),
+        py::arg("codes_t") = py::none(), py::arg("scale_inv") = py::none(), py::arg("colsum") = py::none());
   m.def("layernorm_fwd", &layernorm_fwd);
   m.def("layernorm_bwd", &layernorm_bwd);
   m.def("colsum", &colsum);

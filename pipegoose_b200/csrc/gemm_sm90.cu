@@ -32,20 +32,23 @@ static PFN_encodeTiled get_encode_fn() {
   return fn;
 }
 
-// 2-D bf16 (fp32: f32 = true) tensor map over a row-major [rows, cols] matrix (cols contiguous, leading
-// dimension ld elements) with a [box_rows, box_cols] box and 128-byte swizzle.
+// 2-D tensor map over a row-major [rows, cols] matrix (cols contiguous, leading dimension ld elements) of esize-byte
+// elements (1: FP8 codes as UINT8, 2: bf16, 4: fp32) with a [box_rows, box_cols] box and 128-byte swizzle.
 static int make_tmap_2d(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld,
-                        uint32_t box_rows, uint32_t box_cols, bool f32) {
+                        uint32_t box_rows, uint32_t box_cols, int esize) {
   PFN_encodeTiled enc = get_encode_fn();
   if (!enc) return -1;
   // driver entry points need the primary context bound to the calling thread (autograd worker
   // threads have not necessarily touched the runtime yet)
   cudaFree(nullptr);
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * (f32 ? 4 : 2)};
+  cuuint64_t strides[1] = {ld * esize};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(out, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims,
+  const CUtensorMapDataType dt = esize == 4   ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                 : esize == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                              : CU_TENSOR_MAP_DATA_TYPE_UINT8;
+  CUresult r = enc(out, dt, 2, const_cast<void*>(ptr), dims,
                    strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -62,7 +65,7 @@ static int make_tmap_2d(CUtensorMap* out, const void* ptr, uint64_t rows, uint64
 
 int make_tmap_bf16_2d(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols,
                       uint64_t ld, uint32_t box_rows, uint32_t box_cols) {
-  return make_tmap_2d(out, ptr, rows, cols, ld, box_rows, box_cols, false);
+  return make_tmap_2d(out, ptr, rows, cols, ld, box_rows, box_cols, 2);
 }
 
 // 3-D fp32 tensor map over a contiguous [d2, d1, d0] tensor (d0 contiguous) with a [1, box1, 32] box and 128-byte
@@ -90,9 +93,9 @@ struct TmapKey {
   const void* ptr;
   uint64_t rows, cols, ld;
   uint32_t box_rows;
-  bool f32;
+  int esize;
   bool operator==(const TmapKey& o) const {
-    return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && f32 == o.f32;
+    return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && esize == o.esize;
   }
 };
 struct TmapKeyHash {
@@ -100,24 +103,24 @@ struct TmapKeyHash {
     size_t h = reinterpret_cast<size_t>(k.ptr);
     h ^= k.rows * 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2);
     h ^= k.cols * 0xC2B2AE3D27D4EB4Full + (h << 6) + (h >> 2);
-    h ^= (k.ld * 31 + k.box_rows * 2 + k.f32) + (h << 6) + (h >> 2);
+    h ^= (k.ld * 31 + k.box_rows * 8 + k.esize) + (h << 6) + (h >> 2);
     return h;
   }
 };
 
-// bf16 maps have [box_rows x 64] boxes, fp32 maps (f32 = true) [box_rows x 32]: 128-byte box rows either way
+// [box_rows x 128 / esize] boxes: 128-byte box rows (64 bf16, 32 fp32 or 128 FP8 codes)
 static int cached_tmap(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols,
-                       uint64_t ld, uint32_t box_rows, bool f32 = false) {
+                       uint64_t ld, uint32_t box_rows, int esize = 2) {
   static std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> cache;
   static std::mutex mu;
-  TmapKey key{ptr, rows, cols, ld, box_rows, f32};
+  TmapKey key{ptr, rows, cols, ld, box_rows, esize};
   std::lock_guard<std::mutex> g(mu);
   auto it = cache.find(key);
   if (it != cache.end()) {
     *out = it->second;
     return 0;
   }
-  if (make_tmap_2d(out, ptr, rows, cols, ld, box_rows, f32 ? 32 : 64, f32) != 0) return -1;
+  if (make_tmap_2d(out, ptr, rows, cols, ld, box_rows, 128 / esize, esize) != 0) return -1;
   if (cache.size() > 8192) cache.clear();
   cache.emplace(key, *out);
   return 0;
@@ -139,11 +142,11 @@ struct EpiMaps {
   CUtensorMap out, aux, in;
 };
 
-template <int BN, bool A_MN, bool B_MN, bool TMA_EPI>
+template <int BN, bool A_MN, bool B_MN, bool TMA_EPI, int FMT = FMT_BF16>
 static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tal, const EpiMaps& em,
                       const GemmArgs& args, int max_ctas, cudaStream_t stream) {
   using Cfg = GemmCfg<BN, TMA_EPI>;
-  auto kern = gemm_bf16_kernel<BN, A_MN, B_MN, TMA_EPI>;
+  auto kern = gemm_bf16_kernel<BN, A_MN, B_MN, TMA_EPI, FMT>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e =
@@ -185,16 +188,18 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const CUtens
 // Tile width (and, for fp32-accumulating outputs, a K split) by a wave-quantisation cost model:
 // cost = waves * (k-blocks per work item * BN / efficiency(BN)) + one exposed epilogue.
 // cheap_split: partial sums leave through the TMA epilogue's reduce-adds, which cost what a plain store costs.
-static int pick_bn(int M_rows, int N, int K, int chunks, int ctas, bool allow_split, bool cheap_split, int* k_splits) {
+// kblk: elements of a k-block (BK for bf16, 2 BK for FP8); max_bn: widest tile allowed.
+static int pick_bn(int M_rows, int N, int K, int kblk, int max_bn, int chunks, int ctas, bool allow_split,
+                   bool cheap_split, int* k_splits) {
   const int cand[4] = {256, 192, 128, 64};
   const float eff[4] = {1.0f, 0.93f, 0.82f, 0.55f};  // 128 x BN tiles
-  const int num_kb = (K + BK - 1) / BK;
+  const int num_kb = (K + kblk - 1) / kblk;
   int best = 256;
   float best_cost = 1e30f;
   *k_splits = 1;
   for (int i = 0; i < 4; ++i) {
     const int bn = cand[i];
-    if (bn > 64 && N <= bn / 2) continue;
+    if (bn > max_bn || (bn > 64 && N <= bn / 2)) continue;
     const long tiles = (long)((M_rows + BM - 1) / BM) * ((N + bn - 1) / bn) * chunks;
     const int max_split = allow_split ? 8 : 1;
     for (int s = 1; s <= max_split; ++s) {
@@ -251,6 +256,22 @@ extern "C" int pg_gemm_bf16(const PgGemmDesc* d, cudaStream_t stream) {
   args.ce_valid = d->ce_valid > 0 ? d->ce_valid : d->N;
   args.grad_rs = d->grad_rs;
   args.bias_grad = d->bias_grad;
+  args.a_scale_inv = d->a_scale_inv;
+  args.b_scale_inv = d->b_scale_inv;
+  const bool fp8 = d->fmt != FMT_BF16;
+  const int kblk = fp8 ? 2 * BK : BK;
+  if (fp8 && (d->fmt != FMT_E4M3 && d->fmt != FMT_E5M2)) {
+    fprintf(stderr, "pipegoose_b200: unknown GEMM operand format %d\n", d->fmt);
+    return -1;
+  }
+  if (fp8 && (d->a_mn || d->b_mn || d->num_chunks > 1 || d->n_comm > 0 || d->grad_rs.world > 1 ||
+              d->ce_part != nullptr || (d->flags & (EPI_BGRAD | EPI_SCATTER)) || d->a_scale_inv == nullptr ||
+              d->b_scale_inv == nullptr || (d->K % 16) != 0 || (d->lda % 16) != 0 || (d->ldb % 16) != 0 ||
+              (reinterpret_cast<uintptr_t>(d->A) & 15) != 0 || (reinterpret_cast<uintptr_t>(d->B) & 15) != 0)) {
+    fprintf(stderr, "pipegoose_b200: the FP8 GEMM needs K-major 16-byte-aligned operands (K %% 16 == 0), both scales, "
+                    "one chunk and no fused collective, scatter or bias gradient\n");
+    return -1;
+  }
   if ((args.flags & EPI_BGRAD) &&
       (!d->a_mn || args.bias_grad == nullptr || d->num_chunks > 1 || d->n_comm > 0)) {
     fprintf(stderr, "pipegoose_b200: the fused bias gradient needs an MN-major A, a bias_grad buffer and one chunk\n");
@@ -298,8 +319,9 @@ extern "C" int pg_gemm_bf16(const PgGemmDesc* d, cudaStream_t stream) {
                        !(args.flags & (EPI_GELU | EPI_RESIDUAL | EPI_DGELU | EPI_SCATTER)) &&
                        (reinterpret_cast<uintptr_t>(args.out) & 15) == 0;
   int auto_splits = 1;
-  int bn = pick_bn(chunk_rows, args.N, args.K, args.num_chunks, max_ctas - args.n_comm, allow_split, f32_tma,
-                   &auto_splits);
+  // FP8 promotes each k-block's partial sums into a second set of accumulators: tiles up to 128 wide
+  int bn = pick_bn(chunk_rows, args.N, args.K, kblk, fp8 ? 128 : 256, args.num_chunks, max_ctas - args.n_comm,
+                   allow_split, f32_tma, &auto_splits);
   if (args.ce_part != nullptr && d->block_n <= 0) {
     // the partials are laid out per 256-column tile (two per row and tile): fix the tile width
     bn = 256;
@@ -311,7 +333,7 @@ extern "C" int pg_gemm_bf16(const PgGemmDesc* d, cudaStream_t stream) {
   }
   args.k_splits = (allow_split && d->k_splits > 1) ? d->k_splits : auto_splits;
   {
-    const int num_kb = (args.K + BK - 1) / BK;
+    const int num_kb = (args.K + kblk - 1) / kblk;
     if (args.k_splits > num_kb) args.k_splits = num_kb;
     if (args.k_splits > 1) {
       const int per = (num_kb + args.k_splits - 1) / args.k_splits;
@@ -330,14 +352,15 @@ extern "C" int pg_gemm_bf16(const PgGemmDesc* d, cudaStream_t stream) {
   args.a_local_chunk = -1;
   // A: K-major  -> matrix [M, K] (ld = lda), box [128 rows, 64]
   //    MN-major -> matrix [K, M] (ld = lda), box [64 k-rows, 64]
+  const int op_esize = fp8 ? 1 : 2;
   if (!d->a_mn) {
-    if (cached_tmap(&ta, d->A, d->M, d->K, d->lda, BM) != 0) return -1;
+    if (cached_tmap(&ta, d->A, d->M, d->K, d->lda, BM, op_esize) != 0) return -1;
   } else {
     if (cached_tmap(&ta, d->A, d->K, d->M, d->lda, BK) != 0) return -1;
   }
   const uint64_t b_groups = d->b_chunk_rows > 0 ? (uint64_t)args.num_chunks : 1;  // stacked expert weights
   if (!d->b_mn) {
-    if (cached_tmap(&tb, d->B, d->N * b_groups, d->K, d->ldb, bn) != 0) return -1;
+    if (cached_tmap(&tb, d->B, d->N * b_groups, d->K, d->ldb, bn, op_esize) != 0) return -1;
   } else {
     if (cached_tmap(&tb, d->B, d->K * b_groups, d->N, d->ldb, BK) != 0) return -1;
   }
@@ -367,13 +390,34 @@ extern "C" int pg_gemm_bf16(const PgGemmDesc* d, cudaStream_t stream) {
   EpiMaps em;
   memset(&em, 0, sizeof(em));
   if (f32_tma) {
-    if (cached_tmap(&em.out, args.out, args.M, args.N, args.ldc, 64, true) != 0) return -1;
+    if (cached_tmap(&em.out, args.out, args.M, args.N, args.ldc, 64, 4) != 0) return -1;
     em.aux = em.in = em.out;
   } else if (tma_epi) {
     if (cached_tmap(&em.out, args.out, args.M, args.N, args.ldc, 64) != 0) return -1;
     em.aux = em.in = em.out;
     if (gelu_aux && cached_tmap(&em.aux, args.aux, args.M, args.N, args.ldc, 64) != 0) return -1;
     if (epi_in != nullptr && cached_tmap(&em.in, epi_in, args.M, args.N, in_ld, 64) != 0) return -1;
+  }
+
+  if (fp8) {
+    if (!tma_epi) {
+      fprintf(stderr, "pipegoose_b200: the FP8 GEMM runs the TMA epilogue only: 16-byte-aligned bf16 output, bias, "
+                      "residual and GELU' input (no GELU pre-activation together with an epilogue input), or a plain "
+                      "fp32 output\n");
+      return -1;
+    }
+#define PG_DISPATCH_FP8(FMT)                                                                          \
+  switch (bn) {                                                                                       \
+    case 128: return launch_cfg<128, false, false, true, FMT>(ta, tb, tal, em, args, max_ctas, stream); \
+    case 64: return launch_cfg<64, false, false, true, FMT>(ta, tb, tal, em, args, max_ctas, stream);   \
+    default: fprintf(stderr, "pipegoose_b200: FP8 block_n must be 64 or 128, got %d\n", bn); return -1; \
+  }
+    if (d->fmt == FMT_E4M3) {
+      PG_DISPATCH_FP8(FMT_E4M3)
+    } else {
+      PG_DISPATCH_FP8(FMT_E5M2)
+    }
+#undef PG_DISPATCH_FP8
   }
 
 #define PG_DISPATCH_BN(AMN, BMN, EPI)                                                                    \

@@ -19,6 +19,7 @@
 //                        per-owner arrival counter with a system-scope release.
 // The epilogue applies bias / tanh-GELU (also emitting the pre-activation) /
 // GELU-backward / residual add / fp32 accumulate, so none of those is a separate pass.
+// FP8 operands (FMT, the FP8 linear layers): NT only, TMA epilogue only, per-tensor scales applied in the epilogue.
 #pragma once
 #include "grad_rs.cuh"
 #include "ptx.cuh"
@@ -96,7 +97,15 @@ struct GemmArgs {
   // buffer of the rank that owns its ZeRO-1 slice (local L2 atomics / NVLink peer atomics); grad_rs.world <= 1: off
   PgGradRS grad_rs;
   float* bias_grad;  // EPI_BGRAD: fp32 [M]
+  // FP8 operands (FMT != FMT_BF16): value = code * scale_inv, one fp32 device scalar per operand; the epilogue multiplies
+  // every accumulator by a_scale_inv * b_scale_inv before anything else
+  const float* a_scale_inv;
+  const float* b_scale_inv;
 };
+
+// Operand formats of the kernel.  FP8 (A e4m3 or e5m2, B e4m3) is K-major only and runs the TMA epilogue only: a
+// k-block is 128 codes, i.e. the same 128-byte swizzled rows, stage sizes and descriptors as a 64-wide bf16 k-block.
+enum GemmFmt : int { FMT_BF16 = 0, FMT_E4M3 = 1, FMT_E5M2 = 2 };
 
 constexpr int BM = 128;
 constexpr int BK = 64;
@@ -368,9 +377,11 @@ constexpr int kGemmLightRegs = 40;
 constexpr int kGemmConsumerRegs = 232;
 
 // TMA_EPI selects the epilogue (the host picks the TMA-store one for every bf16-output, single-chunk call with
-// 16-byte-aligned matrices, see gemm_sm90.cu); the producer and the main loop are the same for both.
+// 16-byte-aligned matrices, see gemm_sm90.cu); the producer and the main loop are the same for both.  FMT: the operand
+// format (GemmFmt); FP8 changes the k-block width in elements, the wgmma instruction, the promotion of each k-block's
+// partial sums into the fp32 accumulators and the dequantizing scale.
 // tma_out / tma_aux / tma_in ([64 x 64] boxes, 128B swizzle over out, aux and epi_input()) are read only by it.
-template <int BN, bool A_MN, bool B_MN, bool TMA_EPI>
+template <int BN, bool A_MN, bool B_MN, bool TMA_EPI, int FMT>
 __global__ void __launch_bounds__(kGemmThreads, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a,
                      const __grid_constant__ CUtensorMap tma_b,
@@ -380,6 +391,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
                      const __grid_constant__ CUtensorMap tma_in, const GemmArgs args) {
   using Cfg = GemmCfg<BN, TMA_EPI>;
   constexpr int STAGES = Cfg::kStages;
+  static_assert(FMT == FMT_BF16 || (!A_MN && !B_MN && TMA_EPI), "FP8 operands are K-major and use the TMA epilogue");
+  constexpr int KB = FMT == FMT_BF16 ? BK : 2 * BK;  // elements of a k-block (128-byte rows either way)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -410,7 +423,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
   const int unit_stride = static_cast<int>(gridDim.x) - args.n_comm;
   const int n_blks = (args.N + BN - 1) / BN;
   const int num_tiles = m_blks_per_chunk * n_blks * args.num_chunks;
-  const int num_kb = (args.K + BK - 1) / BK;
+  const int num_kb = (args.K + KB - 1) / KB;
   const int k_splits = args.k_splits > 1 ? args.k_splits : 1;
   const int kb_per_split = (num_kb + k_splits - 1) / k_splits;
   const int num_work = num_tiles * k_splits;  // work item t: tile t % num_tiles, K split t / num_tiles
@@ -539,14 +552,14 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
           uint8_t* sb = smem_b + stage * Cfg::kBBytes;
           mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
           if constexpr (!A_MN) {
-            tma_load_2d(sa, map_a, &full_bar[stage], kb * BK, m0);
+            tma_load_2d(sa, map_a, &full_bar[stage], kb * KB, m0);
           } else {
 #pragma unroll
             for (int i = 0; i < BM / 64; ++i)
               tma_load_2d(sa + i * (BK * 128), map_a, &full_bar[stage], m0 + i * 64, kb * BK);
           }
           if constexpr (!B_MN) {
-            tma_load_2d(sb, &tma_b, &full_bar[stage], kb * BK, n0 + tc.chunk * args.b_chunk_rows);
+            tma_load_2d(sb, &tma_b, &full_bar[stage], kb * KB, n0 + tc.chunk * args.b_chunk_rows);
           } else {
 #pragma unroll
             for (int i = 0; i < BN / 64; ++i)
@@ -676,6 +689,39 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         const int kb_end = min(num_kb, kb_begin + kb_per_split);
         int prev_stage = -1;
         wgmma_fence_regs(acc);
+        if constexpr (FMT != FMT_BF16) {
+          // FP8 wgmma accumulates with less than fp32 precision: each 128-wide k-block is summed by the tensor cores
+          // into `part` alone and then added into the fp32 accumulators (promotion), so that error does not grow
+          // with K.  The stage is released as soon as its k-block retired.
+          float part[BN / 2];
+          for (int kb = kb_begin; kb < kb_end; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t sa = smem_u32(smem_a + stage * Cfg::kABytes) + wg * (64 * 128);
+            const uint32_t sb = smem_u32(smem_b + stage * Cfg::kBBytes);
+            wgmma_fence_regs(part);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BK / WG_K; ++k)  // k32 step k: bytes [32 k, 32 k + 32) of the K-major rows
+              WgmmaFp8<BN, FMT == FMT_E5M2>::mma(part, make_wgmma_desc_sw128(sa + k * 32, 0, 1024),
+                                                 make_wgmma_desc_sw128(sb + k * 32, 0, 1024), k > 0 ? 1u : 0u);
+            wgmma_commit();
+            if constexpr (TMA_EPI) {
+              if (kb == kb_begin && t != unit0 && tid_wg == 0) {
+                tma_store_wait_read<0>();
+                if (has_in) mbar_arrive(epi_empty);
+              }
+            }
+            wgmma_wait<0>();
+            wgmma_fence_regs(part);
+            if (tid_wg == 0) mbar_arrive(&empty_bar[stage]);
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[i] = kb > kb_begin ? acc[i] + part[i] : part[i];
+            if (++stage == STAGES) {
+              stage = 0;
+              phase ^= 1;
+            }
+          }
+        } else {
         for (int kb = kb_begin; kb < kb_end; ++kb) {
           mbar_wait(&full_bar[stage], phase);
           // this warpgroup's 64 rows: the second half of a K-major tile, or the second 64-wide atom of an MN-major one
@@ -709,6 +755,13 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
         if (prev_stage >= 0 && tid_wg == 0) mbar_arrive(&empty_bar[prev_stage]);
+        }
+      }
+      if constexpr (FMT != FMT_BF16) {
+        // dequantize once: the product of the two per-tensor scales (read after pdl_wait: the casts wrote them)
+        const float s = *args.a_scale_inv * *args.b_scale_inv;
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] *= s;
       }
       if constexpr (TMA_EPI) {
         uint8_t* wslots = smem_slots + wg * (BN / 64) * Cfg::kSlotBytes;

@@ -74,6 +74,12 @@ typedef struct PgGemmDesc {
   // wgrad (a_mn): with EPI_BGRAD (256) in flags, bias_grad[m] (fp32 [M]) += sum over k of A[k, m], the bias gradient
   // summed from the dY stages the GEMM already loads
   float* bias_grad;
+  // FP8 operands: fmt 1 = A e4m3, 2 = A e5m2 (B e4m3 in both; 0 = bf16).  A [M, K] and B [N, K] codes, both K-major
+  // (a_mn = b_mn = 0), K % 16 == 0; value = code * scale_inv with one fp32 device scalar per operand.  Only the TMA
+  // epilogue's cases: bf16 out with bias / bias + GELU (+ pre-activation) / bias + residual / GELU', or plain fp32 out.
+  int fmt;
+  const float* a_scale_inv;
+  const float* b_scale_inv;
 } PgGemmDesc;
 
 // ---- attention_sm90.cu
@@ -216,6 +222,14 @@ int pg_adam_strided(float* master, float* m, float* v, float* grad, void* param_
                     float grad_scale, int adamw, int zero_grad, cudaStream_t s);
 int pg_accum_bf16_to_f32(const void* src, float* dst, int64_t n, float scale, int accumulate,
                          cudaStream_t s);
+
+// ---- fp8_cast.cu (per-tensor FP8 casts of the FP8 linear layers; format in fp8_cast.cu)
+// amax (fp32 device scalar) = max |x| over n bf16 elements (n % 8 == 0, x 16-byte aligned)
+int pg_fp8_amax(const void* x, int64_t n, float* amax, cudaStream_t s);
+// x bf16 [R, C] contiguous (C % 8 == 0) -> codes [R, C], codes_t [C, R], scale_inv (fp32 scalar), colsum (fp32 [C], added
+// into), each written when not null; e5m2: 1 for e5m2 codes, 0 for e4m3
+int pg_fp8_cast(const void* x, int R, int C, int e5m2, const float* amax, void* codes, void* codes_t, float* scale_inv,
+                float* colsum, cudaStream_t s);
 
 #ifdef __cplusplus
 }

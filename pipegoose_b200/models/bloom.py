@@ -49,6 +49,16 @@ class BloomConfig:
     position_embedding: str = "alibi"
     n_positions: int = 0
     embedding_layernorm: bool = True
+    # FP8 training of the blocks' four linear layers (qkv, dense, fc1, fc2; forward, dgrad, wgrad) on the FP8 wgmma GEMM:
+    # e4m3 activations and weights, e5m2 gradients, one scale per tensor taken from the tensor being cast (no amax
+    # history: checkpoints, resume and recompute are unchanged).  LayerNorm, attention, GELU, the residual stream,
+    # embeddings, the lm_head and the optimizer (fp32 master weights and main grads) stay as they are.  Needs the native
+    # path (CUDA bf16 model), token counts / widths that are multiples of 16 and a head size the flash kernel runs
+    # (D <= 128, a multiple of 8; D = 80 runs zero-padded as in bf16); refused (ValueError) under tensor
+    # parallelism, with dropout in training and with a replaced MLP (ExpertLayer / fused MoE).  Data parallelism, ZeRO-1,
+    # pipeline stages and recompute="block" take it but have not been run with it on several GPUs.  KV-cached
+    # generate() and ContinuousBatcher keep using the bf16 weights.
+    fp8: bool = False
 
     @classmethod
     def from_hf(cls, hf_config) -> "BloomConfig":
@@ -144,7 +154,19 @@ class BloomBlock(nn.Module):
         self.post_attention_layernorm = nn.LayerNorm(h, eps=self.eps)
         self.mlp = BloomMLP(config)
         self.hidden_dropout = float(getattr(config, "hidden_dropout", 0.0))
+        self.fp8 = bool(getattr(config, "fp8", False))
         self.tp = None  # set by TensorParallel (sequence-parallel communicator)
+
+    def _check_fp8(self) -> None:
+        """``fp8=True`` cases without an FP8 path: refused rather than run in bf16."""
+        if self.tp is not None:
+            raise ValueError("fp8=True does not support tensor parallelism: the fused all-gather / reduce-scatter GEMMs "
+                             "are bf16")
+        if self.training and (getattr(self, "hidden_dropout", 0.0) > 0.0 or getattr(self, "attention_dropout", 0.0) > 0.0):
+            raise ValueError("fp8=True does not support training with dropout > 0 (hidden_dropout / attention_dropout)")
+        if not isinstance(self.mlp, BloomMLP):
+            raise ValueError(f"fp8=True needs the dense BloomMLP; this block's MLP was replaced by "
+                             f"{type(self.mlp).__name__} (ExpertLayer / fused MoE), which has no FP8 path")
 
     def _forward_with_dropout(self, x: torch.Tensor, batch: int, seq: int,
                               seg_start: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -175,6 +197,9 @@ class BloomBlock(nn.Module):
         """``x``: ``[tokens_local, hidden]`` (token-sharded when ``self.tp`` is set).  ``seg_start``: int32 ``[batch, seq]``
         document starts of packed rows (``ops.attention``), the same on every tensor-parallel rank; None: one document
         per row."""
+        if getattr(self, "fp8", False):
+            self._check_fp8()
+            return self._forward_fp8(x, batch, seq, seg_start)
         if self.training and (getattr(self, "hidden_dropout", 0.0) > 0.0 or getattr(self, "attention_dropout", 0.0) > 0.0):
             return self._forward_with_dropout(x, batch, seq, seg_start)
         attn = self.self_attention
@@ -194,6 +219,16 @@ class BloomBlock(nn.Module):
             ln = fused_layer_norm(x, self.post_attention_layernorm.weight, self.post_attention_layernorm.bias, self.eps)
             x = mlp(ln, x)
         return x
+
+    def _forward_fp8(self, x: torch.Tensor, batch: int, seq: int, seg_start: Optional[torch.Tensor]) -> torch.Tensor:
+        attn, mlp = self.self_attention, self.mlp
+        x = PF.attention_sublayer_fp8(x, self.input_layernorm.weight, self.input_layernorm.bias,
+                                      attn.query_key_value.weight, attn.query_key_value.bias, attn.dense.weight,
+                                      attn.dense.bias, attn.alibi_slopes_local(attn.num_heads), self.eps, batch, seq,
+                                      attn.num_heads, attn.head_dim, seg_start)
+        return PF.layernorm_mlp_fp8(x, self.post_attention_layernorm.weight, self.post_attention_layernorm.bias,
+                                    mlp.dense_h_to_4h.weight, mlp.dense_h_to_4h.bias, mlp.dense_4h_to_h.weight,
+                                    mlp.dense_4h_to_h.bias, self.eps)
 
 
 def _alibi_slopes_local(self: BloomAttention, n_head_local: int) -> torch.Tensor:

@@ -14,6 +14,7 @@ row-parallel GEMMs produce a reduce-scatter (fused: GEMM->RS).
 """
 from __future__ import annotations
 
+import math
 from typing import Optional
 
 import torch
@@ -298,6 +299,174 @@ class LayerNormMLP(torch.autograd.Function):
         return dx, dgamma, dbeta, dw1, db1, dw2, db2, None, None
 
 
+# ----------------------------------------------------------------------------------------------
+# FP8 sub-layers (BloomConfig.fp8): the four linear layers of a block on the FP8 GEMM, everything else as above.
+# Per-tensor current scaling (ops.kernels.fp8_quantize): activations and weights e4m3, gradients e5m2.  FP8 wgmma reads
+# both operands K-major, so every cast also writes the transposed codes and every product is the forward (NT) layout:
+#   forward  Y  = X  · Wᵀ : X codes [M, K],  W codes [N, K]
+#   dgrad    dX = dY · W  : dY codes [M, N], Wᵀ codes [K, N]
+#   wgrad    dW = dYᵀ · X : dYᵀ codes [N, M], Xᵀ codes [K, M]
+# The forward saves Wᵀ codes and the GEMM inputs' transposed codes (half the bytes of the bf16 inputs) for backward.
+# Bias gradients are the fp32 column sums of the bf16 dY, summed by its cast; wgrads go through the fp32 TMA epilogue
+# into main_grad with the same acquire_main_grad / notify_grad_ready protocol as the bf16 layers.
+# ----------------------------------------------------------------------------------------------
+def _fp8_cast_grad(dy, bias):
+    """e5m2 codes of ``dy`` and of ``dyᵀ``, ``scale_inv``, and the bias gradient: added into ``bias.main_grad`` by the
+    cast (then ``None``) or returned."""
+    mg = None
+    if bias is not None:
+        if _main_grad(bias) is not None:
+            mg, _ = acquire_main_grad(bias, will_overwrite=False)
+        else:
+            mg = torch.zeros(dy.shape[1], dtype=torch.float32, device=dy.device)
+    c, ct, s = K.fp8_quantize(dy, "e5m2", transpose=True, colsum_into=mg)
+    db = None
+    if bias is not None:
+        if _main_grad(bias) is not None:
+            notify_grad_ready(bias)
+        else:
+            db = mg.to(bias.dtype)
+    return c, ct, s, db
+
+
+def _fp8_wgrad(dy_t, s_dy, x_t, s_x, weight):
+    """``dW = dyᵀ x`` from the transposed codes, into ``weight.main_grad`` (then ``None``) or returned."""
+    mg = _main_grad(weight)
+    if mg is not None and K.grad_rs_for(mg) is None:
+        mg, accumulate = acquire_main_grad(weight, will_overwrite=True)
+        K.gemm_fp8(dy_t, x_t, s_dy, s_x, accum_into=mg, accumulate=accumulate)
+        notify_grad_ready(weight)
+        return None
+    g = torch.empty(dy_t.shape[0], x_t.shape[0], dtype=torch.float32, device=dy_t.device)
+    K.gemm_fp8(dy_t, x_t, s_dy, s_x, accum_into=g)
+    if mg is None:
+        return g.to(weight.dtype)
+    # a main grad reduce-scattered in-kernel (ZeRO-1): the FP8 GEMM has no such epilogue, the fold kernel adds it
+    mg, accumulate = acquire_main_grad(weight, will_overwrite=True)
+    K.accumulate_grad(g, mg, accumulate)
+    notify_grad_ready(weight)
+    return None
+
+
+def _fp8_cast(x):
+    """e4m3 codes, transposed codes and ``scale_inv`` of an activation or weight."""
+    return K.fp8_quantize(x.contiguous(), "e4m3", transpose=True)
+
+
+def _attention_width(D):
+    """``(DP, softmax scale)`` of the flash kernel for head size ``D``: D itself (scale 0: the kernel's 1/sqrt(D)), or
+    heads zero-padded to DP with the true width's scale (``ops.attention._AlibiAttentionPadded``, e.g. D = 80)."""
+    from pipegoose_b200.ops.attention import _native_attention_available, padded_head_dim
+
+    if _native_attention_available(D):
+        return D, 0.0
+    return padded_head_dim(D), 1.0 / math.sqrt(D)
+
+
+class AttentionSubLayerFP8(torch.autograd.Function):
+    """:class:`AttentionSubLayer` (no tensor parallelism) with qkv and dense on the FP8 GEMM.  Head sizes without a
+    flash tile of their own (D = 80) run padded, as :func:`ops.attention.alibi_attention` does."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, wqkv, bqkv, wd, bd, slopes, eps, B, S, n_head, D, seg_start=None):
+        from pipegoose_b200.ops import native
+        from pipegoose_b200.ops.attention import native_seg_start, pad_heads, unpad_heads
+
+        DP, scale = _attention_width(D)
+        ln, mean, rstd = K.layernorm_fwd(x, gamma, beta, eps)
+        ln_c, ln_t, s_ln = _fp8_cast(ln)
+        del ln
+        wq_c, wq_t, s_wq = _fp8_cast(wqkv)
+        qkv = K.gemm_fp8(ln_c, wq_c, s_ln, s_wq, bias=bqkv)
+        del ln_c, wq_c
+        qkv = pad_heads(qkv, n_head, 3, D, DP).contiguous()
+        att_p = torch.empty(B * S, n_head * DP, dtype=qkv.dtype, device=qkv.device)
+        lse = torch.empty(B, n_head, S, dtype=torch.float32, device=qkv.device)
+        seg = native_seg_start(seg_start)
+        native().attention_fwd(qkv, slopes, att_p, lse, B, S, n_head, DP, scale, seg)
+        att_c, att_t, s_att = _fp8_cast(unpad_heads(att_p, n_head, 1, D, DP))
+        wd_c, wd_t, s_wd = _fp8_cast(wd)
+        y = K.gemm_fp8(att_c, wd_c, s_att, s_wd, bias=bd, residual=x)
+        ctx.save_for_backward(x, gamma, beta, wqkv, bqkv, wd, bd, slopes, mean, rstd, ln_t, s_ln, wq_t, s_wq, qkv,
+                              att_p, lse, att_t, s_att, wd_t, s_wd, seg)
+        ctx.dims = (B, S, n_head, D, DP, scale)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        from pipegoose_b200.ops import native
+        from pipegoose_b200.ops.attention import pad_heads, unpad_heads
+
+        (x, gamma, beta, wqkv, bqkv, wd, bd, slopes, mean, rstd, ln_t, s_ln, wq_t, s_wq, qkv, att_p, lse, att_t, s_att,
+         wd_t, s_wd, seg) = ctx.saved_tensors
+        B, S, n_head, D, DP, scale = ctx.dims
+        dy = dy.contiguous()
+        dy_c, dy_t, s_dy, dbd = _fp8_cast_grad(dy, bd)
+        datt = K.gemm_fp8(dy_c, wd_t, s_dy, s_wd)
+        dwd = _fp8_wgrad(dy_t, s_dy, att_t, s_att, wd)
+        del dy_c, dy_t
+        datt = pad_heads(datt, n_head, 1, D, DP).contiguous()
+        dqkv = torch.empty_like(qkv)
+        native().attention_bwd(qkv, slopes, att_p, lse, datt, dqkv, B, S, n_head, DP, scale, seg)
+        del datt
+        dqkv = unpad_heads(dqkv, n_head, 3, D, DP).contiguous()
+        dq_c, dq_t, s_dq, dbqkv = _fp8_cast_grad(dqkv, bqkv)
+        del dqkv
+        dln = K.gemm_fp8(dq_c, wq_t, s_dq, s_wq)
+        dwqkv = _fp8_wgrad(dq_t, s_dq, ln_t, s_ln, wqkv)
+        dx, dgamma, dbeta = _ln_bwd(dln, x, gamma, beta, mean, rstd, dx_extra=dy)
+        return dx, dgamma, dbeta, dwqkv, dbqkv, dwd, dbd, None, None, None, None, None, None, None
+
+
+class LayerNormMLPFP8(torch.autograd.Function):
+    """:class:`LayerNormMLP` (no tensor parallelism) with fc1 and fc2 on the FP8 GEMM: GELU and its pre-activation in
+    the fc1 epilogue, GELU' on the bf16 pre-activation in the fc2 dgrad epilogue."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, w1, b1, w2, b2, eps):
+        ln, mean, rstd = K.layernorm_fwd(x, gamma, beta, eps)
+        ln_c, ln_t, s_ln = _fp8_cast(ln)
+        del ln
+        w1_c, w1_t, s_w1 = _fp8_cast(w1)
+        z = torch.empty(x.shape[0], w1.shape[0], dtype=x.dtype, device=x.device)
+        h1 = K.gemm_fp8(ln_c, w1_c, s_ln, s_w1, bias=b1, gelu=True, aux_out=z)
+        del ln_c, w1_c
+        h1_c, h1_t, s_h1 = _fp8_cast(h1)
+        del h1
+        w2_c, w2_t, s_w2 = _fp8_cast(w2)
+        y = K.gemm_fp8(h1_c, w2_c, s_h1, s_w2, bias=b2, residual=x)
+        ctx.save_for_backward(x, gamma, beta, w1, b1, w2, b2, mean, rstd, ln_t, s_ln, w1_t, s_w1, z, h1_t, s_h1, w2_t,
+                              s_w2)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, gamma, beta, w1, b1, w2, b2, mean, rstd, ln_t, s_ln, w1_t, s_w1, z, h1_t, s_h1, w2_t, s_w2 = ctx.saved_tensors
+        dy = dy.contiguous()
+        dy_c, dy_t, s_dy, db2 = _fp8_cast_grad(dy, b2)
+        dz = K.gemm_fp8(dy_c, w2_t, s_dy, s_w2, dgelu_aux=z)
+        dw2 = _fp8_wgrad(dy_t, s_dy, h1_t, s_h1, w2)
+        del dy_c, dy_t
+        dz_c, dz_t, s_dz, db1 = _fp8_cast_grad(dz, b1)
+        del dz
+        dln = K.gemm_fp8(dz_c, w1_t, s_dz, s_w1)
+        dw1 = _fp8_wgrad(dz_t, s_dz, ln_t, s_ln, w1)
+        dx, dgamma, dbeta = _ln_bwd(dln, x, gamma, beta, mean, rstd, dx_extra=dy)
+        return dx, dgamma, dbeta, dw1, db1, dw2, db2, None
+
+
+def _fp8_check(x, *weights):
+    """The FP8 sub-layers run on the sm_90a kernels only, at shapes the FP8 GEMM takes."""
+    from pipegoose_b200.ops import use_native
+
+    if not use_native(x, *weights):
+        raise ValueError("fp8=True runs on the native path only (CUDA bf16 model and inputs); this model does not")
+    dims = [x.shape[0]] + [d for w in weights for d in w.shape]
+    if any(d % 16 for d in dims):
+        raise ValueError(f"fp8=True needs the token count and every linear layer's width to be multiples of 16, got "
+                         f"{x.shape[0]} tokens and weights {[tuple(w.shape) for w in weights]}")
+
+
 class Linear(torch.autograd.Function):
     """``y = x @ W^T + b`` for any leading shape: wgmma GEMM (bias in the epilogue), dgrad and wgrad
     GEMMs in backward.  Used by the reference-compatible Column/RowParallelLinear layers."""
@@ -540,6 +709,20 @@ def attention_sublayer(x, gamma, beta, wqkv, bqkv, wd, bd, slopes, eps, B, S, n_
     att = alibi_attention(qkv, slopes, B, S, n_head, D, seg_start=seg_start)
     return LinearResidual.apply(att, wd, bd, x, tp)
 
+
+def attention_sublayer_fp8(x, gamma, beta, wqkv, bqkv, wd, bd, slopes, eps, B, S, n_head, D, seg_start=None):
+    """:func:`attention_sublayer` with the qkv and dense GEMMs in FP8 (no tensor parallelism)."""
+    _fp8_check(x, wqkv, wd)
+    if _attention_width(D)[0] == 0 or D % 8:
+        raise ValueError(f"fp8=True needs a head size the flash attention kernel runs (natively or zero-padded: "
+                         f"D <= 128, a multiple of 8), got {D}")
+    return AttentionSubLayerFP8.apply(x, gamma, beta, wqkv, bqkv, wd, bd, slopes, eps, B, S, n_head, D, seg_start)
+
+
+def layernorm_mlp_fp8(x, gamma, beta, w1, b1, w2, b2, eps=1e-5):
+    """:func:`layernorm_mlp` with fc1 and fc2 in FP8 (no tensor parallelism)."""
+    _fp8_check(x, w1, w2)
+    return LayerNormMLPFP8.apply(x, gamma, beta, w1, b1, w2, b2, eps)
 
 def linear_residual(a, weight, bias, residual, tp=None):
     return LinearResidual.apply(a, weight, bias, residual, tp)

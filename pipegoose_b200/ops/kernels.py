@@ -136,6 +136,69 @@ def gemm_tn(dy, x, accum_into: Optional[torch.Tensor] = None, accumulate: bool =
     return g
 
 
+# ----------------------------------------------------------------------------------------------
+# FP8 (per-tensor current scaling) for the FP8 linear layers
+# ----------------------------------------------------------------------------------------------
+FP8_FORMATS = {"e4m3": (torch.float8_e4m3fn, 448.0), "e5m2": (torch.float8_e5m2, 57344.0)}
+
+
+def fp8_quantize_reference(x: torch.Tensor, fmt: str):
+    """The FP8 cast's definition (and the oracle of its kernel): ``x`` -> (codes of ``x``'s shape, fp32 ``scale_inv``
+    of shape ``[1]``) with ``x ~ codes * scale_inv``.  In fp32, with IEEE division (tensor by tensor: torch computes
+    ``scalar / tensor`` as a reciprocal product):
+
+    * ``amax = max |x|``, ``fmax`` = 448 (``"e4m3"``) or 57344 (``"e5m2"``);
+    * ``scale = min(fmax / amax, FLT_MAX)``, 1 when ``amax == 0``; ``code = rn(clamp(x * scale, -fmax, fmax))``;
+    * ``scale_inv = amax / fmax``, 1 when ``amax == 0``, NaN when ``amax`` is not finite (an inf or NaN in a gradient
+      must not turn into finite codes)."""
+    dtype, fmax = FP8_FORMATS[fmt]
+    xf = x.float()
+    amax = xf.abs().amax().reshape(1) if xf.numel() else torch.zeros(1, device=x.device)
+    m = torch.full_like(amax, fmax)
+    zero = amax == 0
+    scale = torch.where(zero, torch.ones_like(amax), torch.fmin(m / amax, torch.full_like(amax, torch.finfo(torch.float32).max)))
+    codes = torch.clamp(xf * scale, -fmax, fmax).to(dtype)
+    scale_inv = torch.where(zero, torch.ones_like(amax), amax / m)
+    scale_inv = torch.where(torch.isfinite(amax), scale_inv, torch.full_like(amax, float("nan")))
+    return codes, scale_inv
+
+
+def fp8_quantize(x: torch.Tensor, fmt: str, codes: bool = True, transpose: bool = False,
+                 colsum_into: Optional[torch.Tensor] = None):
+    """Per-tensor FP8 cast of a contiguous bf16 CUDA matrix ``x [R, C]`` (``C % 8 == 0``) in two kernels (amax, then
+    cast), with no host sync.  Returns ``(codes [R, C] or None, codes_t [C, R] or None, scale_inv [1] fp32)`` in the
+    format of :func:`fp8_quantize_reference`, bit for bit.  ``colsum_into`` (fp32 ``[C]``): the column sums of ``x``
+    (bf16 values, fp32 sums) are added into it by the same pass."""
+    dtype, _ = FP8_FORMATS[fmt]
+    R, C = x.shape
+    ws = torch.empty(2, dtype=torch.float32, device=x.device)   # [amax, scale_inv]
+    c = torch.empty(R, C, dtype=dtype, device=x.device) if codes else None
+    ct = torch.empty(C, R, dtype=dtype, device=x.device) if transpose else None
+    scale_inv = ws[1:]
+    native().fp8_quantize(x, fmt == "e5m2", ws, codes=c, codes_t=ct, scale_inv=scale_inv, colsum=colsum_into)
+    return c, ct, scale_inv
+
+
+def gemm_fp8(a, b, a_scale_inv, b_scale_inv, bias=None, residual=None, gelu=False, aux_out=None, dgelu_aux=None,
+             accum_into: Optional[torch.Tensor] = None, accumulate: bool = False, out=None, block_n: int = 0,
+             k_splits: int = 0):
+    """``out[M, N] = epi(a_scale_inv * b_scale_inv * (a[M, K] @ b[N, K]^T))`` on FP8 codes (``a`` e4m3 or e5m2, ``b``
+    e4m3, both K-major, ``K % 16 == 0``).  bf16 out with bias, tanh-GELU (pre-activation into ``aux_out``), residual
+    or ``* gelu'(dgelu_aux)``; or, with ``accum_into`` (fp32 ``[M, N]``), overwritten (``accumulate=False``) or added
+    into.  There is no fallback: FP8 runs on the sm_90a kernel only."""
+    M, N = a.shape[0], b.shape[0]
+    if accum_into is not None:
+        native().gemm_fp8(a, b, a_scale_inv, b_scale_inv, accum_into.view(M, N), accumulate=accumulate,
+                          block_n=block_n, k_splits=k_splits)
+        return None
+    if out is None:
+        out = torch.empty(M, N, dtype=torch.bfloat16, device=a.device)
+    aux = aux_out if gelu else dgelu_aux
+    native().gemm_fp8(a, b, a_scale_inv, b_scale_inv, out, bias=bias, residual=residual, aux=aux, gelu=gelu,
+                      dgelu=dgelu_aux is not None, block_n=block_n, k_splits=k_splits)
+    return out
+
+
 def colsum(dy, accum_into: Optional[torch.Tensor] = None):
     """Bias gradient: column sums of ``dy`` (accumulated into the fp32 main grad when given)."""
     if use_native(dy):
