@@ -544,6 +544,56 @@ void paged_decode_attention(const torch::Tensor& qkv, torch::Tensor k_pool, torc
                                         cur_stream()) == 0, "paged_decode_attention failed");
 }
 
+// Paged append attention (decode_sm90.cu, speculative verification): row b appends the tokens of qkv [N, H*3*D] rows
+// cu_seqlens[b] .. cu_seqlens[b+1]-1 (1 to 8 of them) at positions pos[b] ..; each writes its k / v into its slot and
+// attends to keys 0 .. its own position; out [N, H*D].  table, cu_seqlens and pos stay on the device: the caller
+// guarantees that every row appends 1 to max_tokens (<= 8) tokens, pos[b] + its tokens - 1 <= max_pos, that table[b]
+// holds pages of the pool for those positions and that no two rows share a page.  max_tokens picks the kernel's query
+// tile.  ticket: int32, at least 8*B*H entries, all zero.
+void paged_append_attention(const torch::Tensor& qkv, torch::Tensor k_pool, torch::Tensor v_pool,
+                            const torch::Tensor& table, const torch::Tensor& cu_seqlens, const torch::Tensor& pos,
+                            int64_t max_pos, int64_t max_tokens, const torch::Tensor& slopes, torch::Tensor out,
+                            torch::Tensor ticket, double softmax_scale) {
+  check_pools(qkv, k_pool, v_pool, "paged_append_attention");
+  PG_CUDA(out); PG_BF16(out); PG_CUDA(slopes); PG_F32(slopes); PG_CUDA(ticket); PG_CUDA(table); PG_CUDA(cu_seqlens);
+  PG_CUDA(pos);
+  TORCH_CHECK(ticket.scalar_type() == torch::kInt32 && table.scalar_type() == torch::kInt32 &&
+              cu_seqlens.scalar_type() == torch::kInt32 && pos.scalar_type() == torch::kInt32,
+              "paged_append_attention: ticket, table, cu_seqlens and pos must be int32");
+  TORCH_CHECK(table.dim() == 2 && table.size(1) >= 1 && table.is_contiguous(),
+              "paged_append_attention: table must be a contiguous [B, max_pages]");
+  const int64_t B = table.size(0), H = k_pool.size(1), D = k_pool.size(3), max_pages = table.size(1);
+  TORCH_CHECK(cu_seqlens.numel() == B + 1 && pos.numel() == B && cu_seqlens.is_contiguous() && pos.is_contiguous(),
+              "paged_append_attention: cu_seqlens must be [B+1] and pos [B] for the B = ", B, " table rows");
+  TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == H * 3 * D && qkv.is_contiguous(),
+              "paged_append_attention: qkv must be a contiguous [N, H*3*D]");
+  const int64_t N = qkv.size(0);
+  TORCH_CHECK(1 <= max_tokens && max_tokens <= 8, "paged_append_attention: max_tokens ", max_tokens,
+              " outside 1 .. 8");
+  TORCH_CHECK(B <= N && N <= max_tokens * B, "paged_append_attention: ", N, " tokens for ", B,
+              " rows: every row appends 1 to max_tokens = ", max_tokens, " tokens");
+  TORCH_CHECK(out.numel() == N * H * D && out.is_contiguous() && slopes.numel() == H,
+              "paged_append_attention: shape mismatch");
+  TORCH_CHECK(ticket.numel() >= 8 * B * H, "ticket must hold at least 8*B*H = ", 8 * B * H, " entries");
+  TORCH_CHECK(0 <= max_pos && max_pos < max_pages * 64, "paged_append_attention: max_pos ", max_pos,
+              " outside the ", max_pages, " pages of a table row");
+  for (const torch::Tensor* t :
+       std::initializer_list<const torch::Tensor*>{&out, &slopes, &ticket, &table, &cu_seqlens, &pos})
+    TORCH_CHECK(t->device() == qkv.device(), "paged_append_attention: tensors on different devices");
+  if (B == 0) return;
+  c10::cuda::CUDAGuard guard(qkv.device());
+  const int splits = pg_decode_splits((int)B, (int)H, (int)max_pos + 1);
+  torch::Tensor part;
+  if (splits > 1) part = torch::empty({B * H * 8 * splits * (D + 2)}, qkv.options().dtype(torch::kFloat32));
+  TORCH_CHECK(pg_paged_append_attention(qkv.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(), table.data_ptr<int>(),
+                                        cu_seqlens.data_ptr<int>(), pos.data_ptr<int>(), slopes.data_ptr<float>(),
+                                        out.data_ptr(), splits > 1 ? part.data_ptr<float>() : nullptr,
+                                        ticket.data_ptr<int>(), (int)B, (int)N, (int)H, (int)D, (int)max_pages,
+                                        (int)max_pos, (int)max_tokens, splits, (float)softmax_scale,
+                                        cur_stream()) == 0,
+              "paged_append_attention failed");
+}
+
 // Paged prefill attention (attention_sm90.cu, PAGED): the new tokens of R sequences packed in qkv [N, H*3*D] (sequence
 // r: rows cu_seqlens[r] .. cu_seqlens[r+1]-1 at positions start[r], ...) attend to keys 0 .. p of their own sequence,
 // read from the pools through table [R, max_pages]; out [N, H*D].  The pools are not written.  cu_seqlens, start and
@@ -874,6 +924,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("paged_decode_attention", &paged_decode_attention, py::arg("qkv"), py::arg("k_pool"), py::arg("v_pool"),
         py::arg("table"), py::arg("pos"), py::arg("max_pos"), py::arg("slopes"), py::arg("out"), py::arg("ticket"),
         py::arg("softmax_scale") = 0.0);
+  m.def("paged_append_attention", &paged_append_attention, py::arg("qkv"), py::arg("k_pool"), py::arg("v_pool"),
+        py::arg("table"), py::arg("cu_seqlens"), py::arg("pos"), py::arg("max_pos"), py::arg("max_tokens"),
+        py::arg("slopes"), py::arg("out"), py::arg("ticket"), py::arg("softmax_scale") = 0.0);
   m.def("paged_prefill_attention", &paged_prefill_attention, py::arg("qkv"), py::arg("k_pool"), py::arg("v_pool"),
         py::arg("table"), py::arg("cu_seqlens"), py::arg("start"), py::arg("max_len"), py::arg("slopes"), py::arg("out"),
         py::arg("softmax_scale"));

@@ -59,13 +59,17 @@ constexpr int kDecTargetCtas = 132 * 4;
 constexpr float kDecLog2e = 1.4426950408889634f;
 constexpr int kPageShift = 6;        // 64 positions per page of the paged pools
 constexpr int kPageSize = 1 << kPageShift;
+constexpr int kAppendMaxTokens = 8;  // most tokens a row appends in one append-attention call
 
 struct DecodeArgs {
   const __nv_bfloat16* qkv;
   __nv_bfloat16* k_cache;
   __nv_bfloat16* v_cache;
   const float* slopes;
-  const int* lead;
+  union {
+    const int* lead;         // contiguous form: [B] leading pads
+    const int* cu_seqlens;   // append form: [B + 1], row b's tokens are qkv rows cu_seqlens[b] .. cu_seqlens[b+1] - 1
+  };
   __nv_bfloat16* out;
   float* part;   // [B*H, splits, D + 2]: (m, l, o[D]) per split (splits > 1)
   int* ticket;   // [B*H], zero between calls
@@ -90,12 +94,13 @@ PG_DEVICE void bf16x8_to_f32(const uint4& r, float* f) {
   }
 }
 
-// The end of both decode kernels: merge the CTA's key groups (lane sub of group grp holds o for dims sub * E ..), then,
-// with one split, store the output, otherwise this split's partial and, in the CTA that takes the last ticket, the
-// merge of all splits.
+// The end of the decode kernels, once per query: merge the CTA's key groups (lane sub of group grp holds o for dims
+// sub * E ..), then, with one split, store the output row `out`, otherwise this split's partial and, in the CTA that
+// takes the last ticket, the merge of all splits.  `bh` indexes the query's ticket and partials.
 template <int D, int NG, int E>
 PG_DEVICE void decode_merge(const DecodeArgs& a, size_t bh, int split, int grp, int sub, bool active, float m, float l,
-                            const float (&o)[E], float* s_m, float* s_l, float (*s_o)[D], int& s_last) {
+                            const float (&o)[E], float* s_m, float* s_l, float (*s_o)[D], int& s_last,
+                            __nv_bfloat16* out) {
   if (sub == 0) {
     s_m[grp] = m;
     s_l[grp] = l;
@@ -117,7 +122,6 @@ PG_DEVICE void decode_merge(const DecodeArgs& a, size_t bh, int split, int grp, 
       O = fmaf(w, s_o[g][d], O);
     }
   }
-  __nv_bfloat16* out = a.out + bh * D;
   if (a.splits == 1) {   // this CTA saw every key, including pos: L > 0
     if (d < D) out[d] = __float2bfloat16(O / L);
     return;
@@ -264,7 +268,147 @@ __global__ void __launch_bounds__(kDecThreads) decode_attention_kernel(const Dec
     m = mx;
   }
 
-  decode_merge<D, NG>(a, bh, split, grp, sub, active, m, l, o, s_m, s_l, s_o, s_last);
+  decode_merge<D, NG>(a, bh, split, grp, sub, active, m, l, o, s_m, s_l, s_o, s_last, a.out + bh * D);
+}
+
+// Paged append attention (speculative verification): row b appends n = cu_seqlens[b+1] - cu_seqlens[b] tokens
+// (1 <= n <= NQ) at positions pos[b] .. pos[b] + n - 1; query i attends to keys 0 .. pos[b] + i.  The layout of
+// decode_attention_kernel<D, true>, with NQ queries per CTA: every key of the chunk is loaded once and scored against
+// all of the row's queries, each with its own online softmax.  Keys pos[b] .. are read from qkv by the one lane group
+// that handles each, which also stores it into its pool slot; no thread reads a slot this launch writes.  Each query
+// then goes through decode_merge with its own ticket and partials (index (b * H + h) * kAppendMaxTokens + i).
+template <int D, int NQ>
+__global__ void __launch_bounds__(kDecThreads) append_attention_kernel(const DecodeArgs a) {
+  constexpr int VEC = D / 8;
+  constexpr int LPK = VEC <= 8 ? 8 : 16;
+  constexpr int KPW = 32 / LPK;
+  constexpr int NG = kDecWarps * KPW;
+  constexpr int U = NQ <= 2 ? kDecUnroll : 2;   // keys in flight per lane group: fewer with more queries (registers)
+  static_assert(D % 8 == 0 && VEC <= 16 && NQ <= kAppendMaxTokens, "head size / queries");
+  __shared__ float s_m[NG], s_l[NG];
+  __shared__ float s_o[NG][D];
+  __shared__ int s_last;
+
+  pdl_launch_dependents();
+  pdl_wait();
+  const int split = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int H = a.H;
+  const int pos = __ldg(a.row_pos + b);
+  const int t0 = __ldg(a.cu_seqlens + b);
+  const int n = __ldg(a.cu_seqlens + b + 1) - t0;
+  const int lane = threadIdx.x & 31;
+  const int sub = lane % LPK;
+  const int grp = (threadIdx.x >> 5) * KPW + lane / LPK;
+  const bool active = sub < VEC;
+
+  const int chunk = (pos + n - 1 + a.splits) / a.splits;   // ceil((pos + n) / splits)
+  const int k0 = split * chunk;
+  const int k1 = min(k0 + chunk, pos + n);
+
+  const size_t tstride = static_cast<size_t>(H) * 3 * D;     // one token of qkv
+  const __nv_bfloat16* tok = a.qkv + static_cast<size_t>(t0) * tstride + static_cast<size_t>(h) * 3 * D;
+  const uint4* kc = reinterpret_cast<const uint4*>(a.k_cache);
+  const uint4* vc = reinterpret_cast<const uint4*>(a.v_cache);
+  const int* tab = a.table + static_cast<size_t>(b) * a.max_pages;
+  auto key_at = [&](int k) -> size_t {
+    return ((static_cast<size_t>(__ldg(tab + (k >> kPageShift))) * H + h) * kPageSize + (k & (kPageSize - 1))) * VEC;
+  };
+
+  float q[NQ][8];
+#pragma unroll
+  for (int j = 0; j < NQ; ++j) {
+    uint4 r = make_uint4(0, 0, 0, 0);
+    if (active && j < n) r = reinterpret_cast<const uint4*>(tok + j * tstride)[sub];
+    bf16x8_to_f32(r, q[j]);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) q[j][i] *= a.scale_log2;
+  }
+  const float slope_log2 = a.slopes[h] * kDecLog2e;
+
+  float m[NQ], l[NQ], o[NQ][8];
+#pragma unroll
+  for (int j = 0; j < NQ; ++j) {
+    m[j] = -INFINITY;
+    l[j] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) o[j][i] = 0.f;
+  }
+  // the trip count is the same for every thread of the CTA: the shuffles below are never divergent
+  for (int kb = k0; kb < k1; kb += NG * U) {
+    uint4 kr[U], vr[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int k = kb + u * NG + grp;
+      kr[u] = vr[u] = make_uint4(0, 0, 0, 0);
+      if (active && k < k1) {
+        if (k >= pos) {   // a new token: from qkv, and into its slot
+          const __nv_bfloat16* t = tok + (k - pos) * tstride;
+          kr[u] = reinterpret_cast<const uint4*>(t + D)[sub];
+          vr[u] = reinterpret_cast<const uint4*>(t + 2 * D)[sub];
+          reinterpret_cast<uint4*>(a.k_cache)[key_at(k) + sub] = kr[u];
+          reinterpret_cast<uint4*>(a.v_cache)[key_at(k) + sub] = vr[u];
+        } else {
+          const size_t at = key_at(k);
+          kr[u] = __ldg(kc + at + sub);
+          vr[u] = __ldg(vc + at + sub);
+        }
+      }
+    }
+    float s[U][NQ];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      float kf[8];
+      bf16x8_to_f32(kr[u], kf);
+      const int k = kb + u * NG + grp;
+#pragma unroll
+      for (int j = 0; j < NQ; ++j) {
+        s[u][j] = -INFINITY;
+        if (j < n) {   // uniform over the CTA
+          float dot = 0.f;
+#pragma unroll
+          for (int i = 0; i < 8; ++i) dot = fmaf(q[j][i], kf[i], dot);
+#pragma unroll
+          for (int off = LPK / 2; off > 0; off >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, off);
+          if (k < k1 && k <= pos + j) s[u][j] = fmaf(slope_log2, static_cast<float>(k - pos - j), dot);
+        }
+      }
+    }
+    float ref[NQ];
+#pragma unroll
+    for (int j = 0; j < NQ; ++j) {
+      float mx = m[j];
+#pragma unroll
+      for (int u = 0; u < U; ++u) mx = fmaxf(mx, s[u][j]);
+      ref[j] = mx == -INFINITY ? 0.f : mx;   // a group with no key yet: keep l = o = 0
+      const float corr = exp2f(m[j] - ref[j]);
+      l[j] *= corr;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) o[j][i] *= corr;
+      m[j] = mx;
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      float vf[8];
+      bf16x8_to_f32(vr[u], vf);
+#pragma unroll
+      for (int j = 0; j < NQ; ++j) {
+        const float p = exp2f(s[u][j] - ref[j]);
+        l[j] += p;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) o[j][i] = fmaf(p, vf[i], o[j][i]);
+      }
+    }
+  }
+
+  const size_t bh = static_cast<size_t>(b) * H + h;
+#pragma unroll
+  for (int j = 0; j < NQ; ++j) {
+    if (j < n) {
+      if (j > 0) __syncthreads();   // the previous query's merge has read the shared buffers
+      decode_merge<D, NG>(a, bh * kAppendMaxTokens + j, split, grp, sub, active, m[j], l[j], o[j], s_m, s_l, s_o,
+                          s_last, a.out + (static_cast<size_t>(t0 + j) * H + h) * D);
+    }
+  }
 }
 
 #define PG_CHECK_LAUNCH(name)                                                       \
@@ -496,7 +640,7 @@ __global__ void __launch_bounds__(kDecThreads) decode_attention_fp8_kernel(const
     m = mx;
   }
 
-  decode_merge<D, NG>(a, bh, split, grp, sub, active, m, l, o, s_m, s_l, s_o, s_last);
+  decode_merge<D, NG>(a, bh, split, grp, sub, active, m, l, o, s_m, s_l, s_o, s_last, a.out + bh * D);
 }
 
 // One thread per 16 codes: (page i, head, slot, K|V, 16-column group) -> 16 bf16 of page dst[i].
@@ -589,6 +733,57 @@ extern "C" int pg_paged_decode_attention(const void* qkv, void* k_pool, void* v_
   a.row_pos = pos;
   a.max_pages = max_pages;
   return launch_decode_d<true>(a, B, D, s);
+}
+
+extern "C" int pg_paged_append_attention(const void* qkv, void* k_pool, void* v_pool, const int* table,
+                                         const int* cu_seqlens, const int* pos, const float* slopes, void* out,
+                                         float* part, int* ticket, int B, int N, int H, int D, int max_pages,
+                                         int max_pos, int max_tokens, int splits, float softmax_scale,
+                                         cudaStream_t s) {
+  if (max_pos < 0 || max_pages < 1 || splits < 1 || max_tokens < 1 || max_tokens > kAppendMaxTokens || N < B ||
+      N > static_cast<long long>(B) * max_tokens || ticket == nullptr || (splits > 1 && part == nullptr))
+    return -1;
+  if (B == 0) return 0;
+  DecodeArgs a;
+  a.qkv = static_cast<const __nv_bfloat16*>(qkv);
+  a.k_cache = static_cast<__nv_bfloat16*>(k_pool);
+  a.v_cache = static_cast<__nv_bfloat16*>(v_pool);
+  a.slopes = slopes;
+  a.cu_seqlens = cu_seqlens;
+  a.out = static_cast<__nv_bfloat16*>(out);
+  a.part = part;
+  a.ticket = ticket;
+  a.H = H;
+  a.capacity = 0;
+  a.pos = max_pos;
+  a.splits = splits;
+  a.scale_log2 = kDecLog2e * (softmax_scale > 0.f ? softmax_scale : 1.0f / sqrtf(static_cast<float>(D)));
+  a.table = table;
+  a.row_pos = pos;
+  a.max_pages = max_pages;
+  a.k_scales = a.v_scales = nullptr;
+  // the query tile: the smallest power of two that holds the longest row (more queries cost registers and keys in
+  // flight for every row)
+  const int most = max_tokens;
+  const dim3 grid(splits, H, B), block(kDecThreads);
+  cudaError_t e;
+#define PG_APPEND_CASE(DD)                                                                      \
+  case DD:                                                                                      \
+    e = most <= 1   ? launch_pdl(append_attention_kernel<DD, 1>, grid, block, 0, s, a)          \
+        : most <= 2 ? launch_pdl(append_attention_kernel<DD, 2>, grid, block, 0, s, a)          \
+        : most <= 4 ? launch_pdl(append_attention_kernel<DD, 4>, grid, block, 0, s, a)          \
+                    : launch_pdl(append_attention_kernel<DD, 8>, grid, block, 0, s, a);         \
+    break;
+  switch (D) {
+    PG_APPEND_CASE(64)
+    PG_APPEND_CASE(80)
+    PG_APPEND_CASE(128)
+    default: return -1;
+  }
+#undef PG_APPEND_CASE
+  if (e != cudaSuccess) return -1;
+  PG_CHECK_LAUNCH("append_attention");
+  return 0;
 }
 
 extern "C" int pg_paged_kv_write(const void* qkv, const int* slot, void* k_pool, void* v_pool, int N, int H, int D,

@@ -117,6 +117,16 @@ int pg_decode_splits(int B, int H, int span);
 int pg_paged_decode_attention(const void* qkv, void* k_pool, void* v_pool, const int* table, const int* pos,
                               const float* slopes, void* out, float* part, int* ticket, int B, int H, int D,
                               int max_pages, int max_pos, int splits, float softmax_scale, cudaStream_t s);
+// Append form (speculative verification): row b appends the n_b = cu_seqlens[b+1] - cu_seqlens[b] tokens (1 <= n_b <= 8,
+// sum N) of qkv [N, H*3*D] at positions pos[b] .. pos[b] + n_b - 1, writing their k / v into their slots; token i
+// attends to keys 0 .. pos[b] + i.  Every key is read once per CTA for all of the row's tokens.  max_pos >= every
+// pos[b] + n_b - 1 sizes the grid (splits from pg_decode_splits(B, H, max_pos + 1)); max_tokens (1 .. 8) >= every n_b
+// picks the query tile (1, 2, 4 or 8 queries per CTA).  Both are host bounds the caller guarantees.  splits > 1: part
+// holds B*H*8*splits*(D+2) floats; ticket is an int32 [B*H*8] array, zero before the call and zero again after it.
+int pg_paged_append_attention(const void* qkv, void* k_pool, void* v_pool, const int* table, const int* cu_seqlens,
+                              const int* pos, const float* slopes, void* out, float* part, int* ticket, int B, int N,
+                              int H, int D, int max_pages, int max_pos, int max_tokens, int splits,
+                              float softmax_scale, cudaStream_t s);
 // Prefill: the k / v of every token n of qkv [N, H*3*D] into pool slot slot[n] (page * 64 + offset), all heads.
 int pg_paged_kv_write(const void* qkv, const int* slot, void* k_pool, void* v_pool, int N, int H, int D,
                       cudaStream_t s);

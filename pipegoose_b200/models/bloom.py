@@ -359,6 +359,24 @@ class BloomModel(nn.Module):
         self.ln_f = nn.LayerNorm(h, eps=config.layer_norm_epsilon)
 
 
+def filter_logits(logits: torch.Tensor, temperature: float, top_k: int, top_p: float) -> torch.Tensor:
+    """The sampling distribution's logits: ``logits [B, V]`` scaled by ``1 / temperature``, then everything outside the
+    top ``top_k`` and outside the nucleus of mass ``top_p`` set to ``-inf``.  Its softmax is what sampling draws from."""
+    if temperature != 1.0:
+        logits = logits / max(float(temperature), 1e-6)
+    if top_k and top_k > 0:
+        kth = logits.topk(min(int(top_k), logits.shape[-1]), dim=-1).values[:, -1:]
+        logits = logits.masked_fill(logits < kth, float("-inf"))
+    if top_p < 1.0:
+        sorted_logits, order = logits.sort(dim=-1, descending=True)
+        probs = sorted_logits.softmax(-1)
+        # drop a token when the mass BEFORE it already reaches top_p (the most likely token always stays)
+        drop = (probs.cumsum(-1) - probs) >= top_p
+        sorted_logits = sorted_logits.masked_fill(drop, float("-inf"))
+        logits = torch.full_like(logits, float("-inf")).scatter(-1, order, sorted_logits)
+    return logits
+
+
 class BloomForCausalLM(nn.Module):
     base_model_prefix = "transformer"
 
@@ -583,19 +601,8 @@ class BloomForCausalLM(nn.Module):
         top-k / nucleus-filtered) distribution.  Sampled tokens are made identical on every tensor-parallel rank."""
         if not do_sample:
             return logits.argmax(-1)
-        if temperature != 1.0:
-            logits = logits / max(float(temperature), 1e-6)
-        if top_k and top_k > 0:
-            kth = logits.topk(min(int(top_k), logits.shape[-1]), dim=-1).values[:, -1:]
-            logits = logits.masked_fill(logits < kth, float("-inf"))
-        if top_p < 1.0:
-            sorted_logits, order = logits.sort(dim=-1, descending=True)
-            probs = sorted_logits.softmax(-1)
-            # drop a token when the mass BEFORE it already reaches top_p (the most likely token always stays)
-            drop = (probs.cumsum(-1) - probs) >= top_p
-            sorted_logits = sorted_logits.masked_fill(drop, float("-inf"))
-            logits = torch.full_like(logits, float("-inf")).scatter(-1, order, sorted_logits)
-        nxt = torch.multinomial(logits.softmax(-1), 1, generator=generator).squeeze(-1)
+        nxt = torch.multinomial(filter_logits(logits, temperature, top_k, top_p).softmax(-1), 1,
+                                generator=generator).squeeze(-1)
         if self.tp is not None and self.tp.size > 1:
             import torch.distributed as dist
 
@@ -711,14 +718,20 @@ class BloomForCausalLM(nn.Module):
           ``positions`` are absolute, ``slot`` is each token's pool slot, ``table`` (int32 ``[R, max_pages]``) each
           sequence's pages and ``max_len >=`` its suffix length.  Every layer stores the new keys and values, then the
           suffix attends to the whole sequence through the pools.  Returns the logits at ``last``: ``[R, V]``.
+        - append (``cu_seqlens`` given without ``start``): R sequences append 1 .. ``APPEND_MAX_TOKENS`` tokens each,
+          packed back to back as above; ``positions`` are absolute, ``table`` (int32 ``[R, max_pages]``) holds each
+          sequence's pages, ``max_pos >=`` every appended position and ``max_len >=`` every sequence's appended
+          tokens (0: derived, see ``alibi_paged_append_attention``).  Every layer writes the new keys and values and
+          attends through the paged append-attention op.  Returns the logits of every token: ``[N, V]``.
 
         FP8 pools (``float8_e4m3fn``) come with fp32 ``k_scales`` / ``v_scales`` ``[n_layer, num_pages, n_head, 64]``;
         a prefill with cached prefixes then also takes ``stage = (num_pages, src, dst, slot, table)``, the device form of
         :func:`~pipegoose_b200.ops.attention.fp8_prefill_staging` (``table`` as ``[R, width]``), which the kernel path
         reads through one bf16 staging pool shared by all layers.
 
-        CUDA bf16 models with head size 64, 80 or 128 run the flash / paged decode / paged prefill kernels; otherwise
-        (CPU, fp32, other head sizes) their PyTorch references run, over FP8 pools too."""
+        CUDA bf16 models with head size 64, 80 or 128 run the flash / paged decode / paged prefill / append kernels;
+        otherwise (CPU, fp32, other head sizes) their PyTorch references run, over FP8 pools too (append: not over FP8
+        pools)."""
         from pipegoose_b200.ops import attention as A
 
         cfg = self.config
@@ -729,7 +742,10 @@ class BloomForCausalLM(nn.Module):
         write = A.paged_kv_write if native else A.paged_kv_write_reference
         decode = A.alibi_paged_decode_attention if native else A.alibi_paged_decode_attention_reference
         prefill = A.alibi_paged_prefill_attention if native else A.paged_prefill_attention_fp32
+        append = A.alibi_paged_append_attention if native else A.alibi_paged_append_attention_reference
         pos_emb = self.transformer.position_embeddings.weight[positions.long()] if _learned(cfg) else None
+        # append: each sequence's first new position
+        first = positions[cu_seqlens[:-1].long()] if cu_seqlens is not None and start is None else None
         staging = None
         if native and k_scales is not None and start is not None:
             if stage is None:
@@ -751,6 +767,9 @@ class BloomForCausalLM(nn.Module):
                     scales["stage"] = staging
                 return prefill(qkv, k_pools[li], v_pools[li], table, cu_seqlens, start, max_len, slopes, D,
                                **scales).view(1, N, -1)
+            if cu_seqlens is not None:
+                return append(qkv, k_pools[li], v_pools[li], table, cu_seqlens, first, max_pos, slopes, D,
+                              max_tokens=max_len).view(1, N, -1)
             return decode(qkv, k_pools[li], v_pools[li], table, positions, max_pos, slopes, D, **scales).view(1, N, -1)
 
         x = self._inference_layers(self._inference_embed(ids.view(1, N), pos_emb), attend)[0]

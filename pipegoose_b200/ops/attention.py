@@ -502,6 +502,90 @@ def paged_prefill_attention_fp32(qkv: torch.Tensor, k_pool: torch.Tensor, v_pool
     return out.reshape(N, n_head * D).to(qkv.dtype)
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# Append to paged pools (speculative verification, ``pipegoose_b200.serving``).
+#
+# Row r of ``table`` appends ``n_r = cu_seqlens[r+1] - cu_seqlens[r]`` tokens, ``1 <= n_r <= APPEND_MAX_TOKENS``,
+# packed in ``qkv [N, n_head*3*D]`` at positions ``pos[r] .. pos[r] + n_r - 1``.  The op writes their keys and values
+# into their slots, and query i of row r attends to keys ``0 .. pos[r] + i`` with ``q.k * scale + slope[head] *
+# (k - (pos[r] + i))``.  ``max_pos`` is a host integer ``>= pos[r] + n_r - 1`` for every row: it sizes the grid only.
+# ``max_tokens`` is a host integer ``>= n_r`` for every row: it picks the kernel's query tile.  Like the decode op, the
+# kernel reads ``table``, ``cu_seqlens`` and ``pos`` on the device only and trusts them; the row lengths, ``max_pos``
+# and ``max_tokens`` are checked against them when they are host tensors.  Its reference is the prefill reference after
+# the pool write.  FP8 pools are not supported.
+# ---------------------------------------------------------------------------------------------------------------------
+
+APPEND_MAX_TOKENS = 8
+
+
+def _append_tile(cu_seqlens: torch.Tensor, pos: torch.Tensor, max_pos: int, max_tokens: int, N: int, B: int) -> int:
+    """Checks what the host can see and returns the bound on the rows' token counts: ``max_tokens``, or when it is 0
+    the longest row of host ``cu_seqlens`` (of device ones: ``N - B + 1``, every row appending at least one token)."""
+    if not 0 <= max_tokens <= APPEND_MAX_TOKENS:
+        raise ValueError(f"max_tokens {max_tokens} is outside 1 .. {APPEND_MAX_TOKENS} (0: from cu_seqlens)")
+    if cu_seqlens.is_cuda or pos.is_cuda or B == 0:
+        return max_tokens or max(1, min(APPEND_MAX_TOKENS, N - B + 1))
+    n = cu_seqlens[1:] - cu_seqlens[:-1]
+    if not bool(((n >= 1) & (n <= APPEND_MAX_TOKENS)).all()):
+        raise ValueError(f"every row appends 1 .. {APPEND_MAX_TOKENS} tokens, got {n.tolist()}")
+    longest = int(n.max())
+    if max_tokens and longest > max_tokens:
+        raise ValueError(f"max_tokens {max_tokens} is smaller than the longest row ({longest} tokens)")
+    last = int((pos.long() + n.long()).max()) - 1
+    if last > max_pos:
+        raise ValueError(f"max_pos {max_pos} is smaller than the last appended position {last}")
+    return max_tokens or longest
+
+
+def alibi_paged_append_attention_reference(qkv: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
+                                           table: torch.Tensor, cu_seqlens: torch.Tensor, pos: torch.Tensor,
+                                           max_pos: int, slopes: torch.Tensor, D: int, softmax_scale: float = 0.0,
+                                           max_tokens: int = 0) -> torch.Tensor:
+    """PyTorch form of :func:`alibi_paged_append_attention` for any head size (CPU path, test oracle, and the model's
+    path where no kernel has its head size): :func:`paged_kv_write_reference` of the new tokens, then
+    :func:`paged_prefill_attention_fp32` from ``start = pos``.  Reads ``cu_seqlens`` and ``pos`` on the host."""
+    if k_pool.dtype == torch.float8_e4m3fn:
+        raise ValueError("append attention does not support FP8 pools")
+    _check_max_pos(max_pos, table)
+    B = table.shape[0]
+    cu_seqlens, pos = cu_seqlens.cpu(), pos.cpu()
+    longest = _append_tile(cu_seqlens, pos, max_pos, max_tokens, qkv.shape[0], B)
+    cu, st = cu_seqlens.tolist(), pos.tolist()
+    rows = table.cpu().tolist()
+    slot = [rows[r][p // PAGE_SIZE] * PAGE_SIZE + p % PAGE_SIZE
+            for r in range(B) for p in range(st[r], st[r] + cu[r + 1] - cu[r])]
+    paged_kv_write_reference(qkv, torch.tensor(slot, dtype=torch.long), k_pool, v_pool, D)
+    return paged_prefill_attention_fp32(qkv, k_pool, v_pool, table, cu_seqlens, pos, longest, slopes, D,
+                                        softmax_scale)
+
+
+def alibi_paged_append_attention(qkv: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, table: torch.Tensor,
+                                 cu_seqlens: torch.Tensor, pos: torch.Tensor, max_pos: int, slopes: torch.Tensor,
+                                 D: int, softmax_scale: float = 0.0, max_tokens: int = 0) -> torch.Tensor:
+    """Append the tokens of every row to the paged pools and attend (section comment above): returns
+    ``[N, n_head*D]``.  CUDA bf16 inputs run ``append_attention_kernel`` (``csrc/decode_sm90.cu``, D in 64 / 80 / 128);
+    otherwise :func:`alibi_paged_append_attention_reference` runs.  ``max_tokens`` (1 .. 8) is a host bound on every
+    row's token count that picks the kernel's query tile (1, 2, 4 or 8 queries per CTA, each costing registers for
+    every row); 0 takes the longest row of host ``cu_seqlens``, or ``N - B + 1`` for device ones."""
+    if not use_native(qkv):
+        return alibi_paged_append_attention_reference(qkv, k_pool, v_pool, table, cu_seqlens, pos, max_pos, slopes, D,
+                                                      softmax_scale, max_tokens)
+    if k_pool.dtype == torch.float8_e4m3fn:
+        raise ValueError("append attention does not support FP8 pools")
+    if D not in DECODE_HEAD_DIMS:
+        raise ValueError(f"the append-attention kernel has no head size {D} (supported: {DECODE_HEAD_DIMS})")
+    _check_max_pos(max_pos, table)
+    B, n_head = table.shape[0], k_pool.shape[1]
+    tile = _append_tile(cu_seqlens, pos, max_pos, max_tokens, qkv.shape[0], B)
+    out = torch.empty(qkv.shape[0], n_head * D, dtype=qkv.dtype, device=qkv.device)
+    native().paged_append_attention(qkv.contiguous(), k_pool, v_pool, table.to(torch.int32).contiguous(),
+                                    cu_seqlens.to(qkv.device, torch.int32).contiguous(),
+                                    pos.to(qkv.device, torch.int32).contiguous(), int(max_pos), tile,
+                                    slopes.float().contiguous(), out,
+                                    _decode_ticket(APPEND_MAX_TOKENS * B * n_head, qkv.device), softmax_scale)
+    return out
+
+
 def fp8_prefill_staging(pages, cached, lengths):
     """Host plan of a prefill with cached prefixes over FP8 pools.  Sequence r has pool pages ``pages[r]``, its first
     ``cached[r]`` positions (a multiple of PAGE_SIZE) in the pools and ``lengths[r]`` positions in all; it gets staging

@@ -12,7 +12,7 @@ until it finishes, so nothing is ever preempted, and return to the free list in 
 
 A step is either one prefill of newly admitted prompts, packed into one row of at most ``max_prefill_tokens`` tokens
 (a longer prompt runs alone) through the document-masked flash kernel, or one decode of every running sequence
-through the paged split-KV decode kernel.  Tokens are chosen with the model's ``_select_token``, one call per group of
+through the paged split-KV decode kernel (or, with speculative decoding, a verify step: below).  Tokens are chosen with the model's ``_select_token``, one call per group of
 requests that share sampling parameters.  A step makes one host-to-device upload (tokens, positions and page tables,
 shared by all layers) and one device-to-host transfer (the chosen tokens).
 
@@ -40,7 +40,23 @@ prefill with hits dequantizes the sequences' cached pages into a bf16 staging po
 and runs the paged prefill kernel on it.  A scale belongs to its page slot, so prefix sharing, reference counting and
 eviction are unchanged.  Accuracy on trained checkpoints is not verified here.
 
-Limits: sampled tokens depend on which requests share a step (the random stream is consumed per group);
+Speculative decoding (``num_speculative_tokens=k``, 0 .. 7, off by default; refused with FP8 pools): before a decode
+step every running request drafts up to k tokens by prompt lookup, the tokens that followed the most recent earlier
+occurrence of its last ``SPEC_NGRAM_SIZES`` = 3 (else 2) tokens, found in a per-request n-gram index updated with
+each new token.  A draft never exceeds ``max_new_tokens - generated - 1`` tokens, so the step writes only inside the
+pages reserved at admission.  If no request has a draft, the step is the decode step above.  Otherwise it is a verify
+step: every running request appends its last token and its drafts (one token without a draft) through the paged
+append-attention kernel, which writes their keys and values and returns the logits of every token; each request
+keeps the drafts ``verify_drafts`` accepts plus one more token, cut at ``eos_token_id`` and ``max_new_tokens``.
+Greedy requests accept a draft while it is the arg-max; sampled requests use rejection sampling, which keeps the
+distribution of non-speculative sampling.  Still one upload and one device-to-host transfer per step.  Invariant:
+positions ``0 .. len(tokens) - 2`` of a request are always valid in its pages.  Rejected drafts leave stale keys and
+values behind the accepted ones; the next step of that request writes those positions before any query reads them,
+and ``_release`` indexes only the valid positions.  ``speculative_proposed_tokens`` counts the drafts verified and
+``speculative_accepted_tokens`` the accepted drafts that were emitted (not those cut off after an eos).
+
+Limits: sampled tokens depend on which requests share a step (the random stream is consumed per group; in a verify
+step a group takes one uniform number per token row, then one draw per row without the draft, then one per row);
 an ``ExpertLayer`` capacity limit counts the tokens of one step, as in ``generate()`` (with prefix caching, cached keys
 and values were computed in another step, so with a limit that binds they can differ from a recomputation by more than
 rounding).  Tensor-parallel, pipelined and fused NVLink MoE models are refused.
@@ -54,7 +70,38 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
-from pipegoose_b200.ops.attention import PAGE_SIZE, fp8_prefill_staging
+from pipegoose_b200.ops.attention import APPEND_MAX_TOKENS, PAGE_SIZE, fp8_prefill_staging
+
+SPEC_NGRAM_SIZES = (3, 2)                           # trailing n-gram sizes the drafter looks up, longest first
+MAX_SPECULATIVE_TOKENS = APPEND_MAX_TOKENS - 1      # drafts per request and step: with the last token, one append
+
+
+class _NgramIndex:
+    """Prompt-lookup drafting for one token list: for every n in ``SPEC_NGRAM_SIZES``, the position of the token that
+    followed the most recent occurrence of each n-gram.  ``update`` indexes the tokens appended since its last call, so
+    drafting costs O(new tokens) per step, not O(sequence length)."""
+
+    def __init__(self):
+        self.index = {n: {} for n in SPEC_NGRAM_SIZES}
+        self.seen = 0
+
+    def update(self, tokens: List[int]) -> None:
+        for t in range(max(self.seen, 1), len(tokens)):          # token t follows the n-gram tokens[t-n:t]
+            for n in SPEC_NGRAM_SIZES:
+                if t >= n:
+                    self.index[n][tuple(tokens[t - n:t])] = t
+        self.seen = len(tokens)
+
+    def draft(self, tokens: List[int], k: int) -> List[int]:
+        """Up to ``k`` tokens that followed the most recent earlier occurrence of the trailing n-gram of ``tokens``
+        (the longest size that has one), ``[]`` if none.  ``update(tokens)`` comes first."""
+        if k <= 0:
+            return []
+        for n in SPEC_NGRAM_SIZES:
+            f = self.index[n].get(tuple(tokens[-n:])) if len(tokens) > n else None
+            if f is not None:
+                return tokens[f:f + k]
+        return []
 
 
 @dataclass
@@ -67,6 +114,7 @@ class _Request:
     eos_token_id: Optional[int]
     pages: List[int] = field(default_factory=list)
     cached: int = 0            # prompt positions served from the prefix cache (a multiple of the page size)
+    ngrams: Optional[_NgramIndex] = None      # speculative decoding only
 
     @property
     def pages_needed(self) -> int:
@@ -82,11 +130,13 @@ class ContinuousBatcher:
     ``generator``: random stream of sampled requests.
     ``prefix_caching``: reuse the pages of earlier prompts that share a prefix (module docstring).
     ``kv_cache_dtype``: ``None`` keeps the pools in the model's dtype, ``torch.float8_e4m3fn`` stores them in FP8 with
-    per-position scales (module docstring)."""
+    per-position scales (module docstring).
+    ``num_speculative_tokens``: most prompt-lookup drafts per request and decode step, 0 .. 7 (module docstring); 0
+    turns speculation off."""
 
     def __init__(self, model, max_cache_tokens: int, max_prefill_tokens: int = 8192,
                  generator: Optional[torch.Generator] = None, prefix_caching: bool = False,
-                 kv_cache_dtype: Optional[torch.dtype] = None):
+                 kv_cache_dtype: Optional[torch.dtype] = None, num_speculative_tokens: int = 0):
         from pipegoose_b200.models.bloom import BloomMLP, _decodes_incrementally
 
         if getattr(model, "tp", None) is not None:
@@ -102,6 +152,14 @@ class ContinuousBatcher:
             raise ValueError(f"kv_cache_dtype must be None or torch.float8_e4m3fn, got {kv_cache_dtype}")
         if max_prefill_tokens < 1:
             raise ValueError(f"max_prefill_tokens must be at least 1, got {max_prefill_tokens}")
+        if not 0 <= num_speculative_tokens <= MAX_SPECULATIVE_TOKENS:
+            raise ValueError(f"num_speculative_tokens must be in 0 .. {MAX_SPECULATIVE_TOKENS}, got "
+                             f"{num_speculative_tokens}")
+        if num_speculative_tokens and kv_cache_dtype is not None:
+            raise ValueError("speculative decoding does not support FP8 KV-cache pools")
+        self.num_speculative_tokens = int(num_speculative_tokens)
+        self.speculative_proposed_tokens = 0                      # drafts verified
+        self.speculative_accepted_tokens = 0                      # accepted drafts emitted
         cfg = model.config
         self.model = model
         self.max_prefill_tokens = int(max_prefill_tokens)
@@ -163,14 +221,18 @@ class ContinuousBatcher:
     def step(self) -> List[Tuple[int, List[int]]]:
         """One prefill or one decode step; returns ``(rid, prompt + new tokens)`` of the requests that finished."""
         self._admit()
-        reqs, logits = self._forward()
-        if not reqs:
-            return []
-        chosen = self._select(reqs, logits)
+        spec = self._speculate() if self.num_speculative_tokens and not self._admitted else None
+        if spec is not None:
+            reqs, emitted = spec
+        else:
+            reqs, logits = self._forward()
+            if not reqs:
+                return []
+            emitted = [[t] for t in self._select(reqs, logits)]
         done = []
-        for r, t in zip(reqs, chosen):
-            r.tokens.append(t)
-            if len(r.tokens) - r.prompt_len == r.max_new_tokens or t == r.eos_token_id:
+        for r, new in zip(reqs, emitted):
+            r.tokens += new
+            if len(r.tokens) - r.prompt_len == r.max_new_tokens or new[-1] == r.eos_token_id:
                 if self.prefix_caching:
                     self._release(r)
                 else:
@@ -353,3 +415,95 @@ class ContinuousBatcher:
             picks.append(self.model._select_token(logits[i:i + n], do_sample, temperature, top_k, top_p, self.generator))
             i += n
         return torch.cat(picks).tolist()
+
+    # ------------------------------------------------------------------ speculative decoding
+    def _draft(self, r: _Request) -> List[int]:
+        """Prompt-lookup drafts of a running request, at most ``max_new_tokens - generated - 1`` of them so that every
+        position the step writes lies in the pages reserved at admission."""
+        if r.ngrams is None:
+            r.ngrams = _NgramIndex()
+        r.ngrams.update(r.tokens)
+        budget = r.max_new_tokens - (len(r.tokens) - r.prompt_len) - 1
+        return r.ngrams.draft(r.tokens, min(self.num_speculative_tokens, budget))
+
+    def _speculate(self) -> Optional[Tuple[List[_Request], List[List[int]]]]:
+        """A verify step: every running request appends its last token and its drafts through the paged append
+        kernel, and keeps the drafts verification accepts plus one more token.  None when no request has a draft: the
+        step is then the plain decode step."""
+        reqs = sorted(self._running, key=lambda r: r.sampling)
+        drafts = [self._draft(r) for r in reqs]
+        if not any(drafts):
+            return None
+        self._running = []
+        width = max(len(r.pages) for r in reqs)
+        ids, positions, cu, table = [], [], [0], []
+        for r, d in zip(reqs, drafts):
+            p = len(r.tokens) - 1
+            ids += [r.tokens[-1]] + d
+            positions += range(p, p + 1 + len(d))
+            cu.append(len(ids))
+            table += r.pages + [0] * (width - len(r.pages))
+        ids, positions, cu, table = self._upload([ids, positions, cu, table])
+        logits = self.model._paged_logits(ids, positions, self.k_pools, self.v_pools, table=table.view(len(reqs), width),
+                                          max_pos=max(len(r.tokens) - 1 + len(d) for r, d in zip(reqs, drafts)),
+                                          cu_seqlens=cu, max_len=1 + max(len(d) for d in drafts))
+        emitted = verify_drafts([r.sampling for r in reqs], drafts, ids, logits.float(), self.generator)
+        for r, d, new in zip(reqs, drafts, emitted):
+            accepted = len(new) - 1                      # the drafts come first, then one token of the verifier
+            room = r.max_new_tokens - (len(r.tokens) - r.prompt_len)
+            new[:] = new[:room]
+            if r.eos_token_id in new:
+                del new[new.index(r.eos_token_id) + 1:]
+            self.speculative_proposed_tokens += len(d)
+            self.speculative_accepted_tokens += min(accepted, len(new))     # accepted drafts that are emitted
+        return reqs, emitted
+
+
+def verify_drafts(samplings: List[Tuple], drafts: List[List[int]], ids: torch.Tensor, logits: torch.Tensor,
+                  generator: Optional[torch.Generator] = None) -> List[List[int]]:
+    """The tokens each request of a verify step emits: its accepted drafts, then one more token, chosen at the first
+    rejected draft or after the last one.  ``samplings`` are the requests' sampling tuples (equal ones adjacent);
+    ``ids`` / ``logits [N, V]`` are the step's token rows, each request's last token and then its ``drafts``, so row
+    i of a request scores the draft ``ids[i + 1]``.
+
+    Greedy requests accept a draft while it equals the arg-max, and emit the arg-max where they stop.  Sampled
+    requests accept draft x at row i with probability p_i(x), where p_i is the filtered distribution
+    (``filter_logits``) non-speculative sampling draws from; on a rejection they draw from p_i without x,
+    renormalised, and after the last draft from p_i.  The drafts are deterministic, so the emitted tokens follow the
+    distribution of non-speculative sampling.  Per sampled group, the random stream gives one uniform number per row,
+    then one draw per row from the distribution without the draft, then one per row from p_i.  One device-to-host
+    transfer serves all groups."""
+    from pipegoose_b200.models.bloom import filter_logits
+
+    target = torch.cat([ids[1:], ids[-1:]]).long().view(-1, 1)
+    groups = [(key, len(list(g))) for key, g in itertools.groupby(samplings)]
+    outs, row, r0 = [], 0, 0
+    for key, n in groups:
+        m = sum(1 + len(d) for d in drafts[r0:r0 + n])
+        lg, t = logits[row:row + m], target[row:row + m]
+        if not key[0]:
+            a = lg.argmax(-1)
+            outs.append(torch.stack([(a == t.view(-1)).long(), a, a], 1))
+        else:
+            p = filter_logits(lg, *key[1:]).softmax(-1)
+            accept = torch.rand(m, device=p.device, generator=generator) < p.gather(-1, t).view(-1)
+            rest = p.scatter(-1, t, 0.0)
+            rest = torch.where(rest.sum(-1, keepdim=True) > 0, rest, p)      # p(x) = 1: x is never rejected
+            outs.append(torch.stack([accept.long(), torch.multinomial(rest, 1, generator=generator).view(-1),
+                                     torch.multinomial(p, 1, generator=generator).view(-1)], 1))
+        row += m
+        r0 += n
+    verdicts = torch.cat(outs).tolist()          # per row: (draft accepted, token if not, token after the last draft)
+    emitted, row = [], 0
+    for d in drafts:
+        new = []
+        for j, x in enumerate(d):
+            ok, other, _ = verdicts[row + j]
+            new.append(x if ok else other)
+            if not ok:
+                break
+        else:
+            new.append(verdicts[row + len(d)][2])
+        emitted.append(new)
+        row += 1 + len(d)
+    return emitted
