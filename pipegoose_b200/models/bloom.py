@@ -703,7 +703,7 @@ class BloomForCausalLM(nn.Module):
                       max_pos: int = 0, cu_seqlens: Optional[torch.Tensor] = None,
                       start: Optional[torch.Tensor] = None, max_len: int = 0,
                       k_scales: Optional[torch.Tensor] = None, v_scales: Optional[torch.Tensor] = None,
-                      stage: Optional[tuple] = None) -> torch.Tensor:
+                      stage: Optional[tuple] = None, n_dec: Optional[int] = None) -> torch.Tensor:
         """Inference-only forward of a set of sequences over paged KV pools (``pipegoose_b200.serving``); ``ids`` and
         ``positions`` (each token's position in its own sequence) are ``[N]``, ``k_pools`` / ``v_pools`` are
         ``[n_layer, num_pages, n_head, 64, D]``.  Three modes:
@@ -723,11 +723,19 @@ class BloomForCausalLM(nn.Module):
           sequence's pages, ``max_pos >=`` every appended position and ``max_len >=`` every sequence's appended
           tokens (0: derived, see ``alibi_paged_append_attention``).  Every layer writes the new keys and values and
           attends through the paged append-attention op.  Returns the logits of every token: ``[N, V]``.
+        - mixed (``n_dec`` given, chunked prefill): ``n_dec`` decode tokens (one per sequence, as in decode mode)
+          followed by prompt chunks of R sequences (as in the prefill with cached prefixes: ``cu_seqlens`` counts the
+          chunk rows from 0, ``start[r]`` is chunk r's first position, ``slot`` holds the chunk tokens' pool slots).
+          ``table`` (int32 ``[n_dec + R, max_pages]``) holds the decode rows' pages, then the chunks'; ``max_pos`` bounds
+          the decode positions and ``max_len`` the chunk lengths.  Every layer runs the decode rows through the paged
+          decode op (which writes their keys and values), writes the chunks' keys and values and runs the chunks
+          through the paged prefill op; the two touch disjoint pages.  Returns the logits at the rows ``last`` (indices
+          into all N rows): ``[len(last), V]``.
 
         FP8 pools (``float8_e4m3fn``) come with fp32 ``k_scales`` / ``v_scales`` ``[n_layer, num_pages, n_head, 64]``;
         a prefill with cached prefixes then also takes ``stage = (num_pages, src, dst, slot, table)``, the device form of
         :func:`~pipegoose_b200.ops.attention.fp8_prefill_staging` (``table`` as ``[R, width]``), which the kernel path
-        reads through one bf16 staging pool shared by all layers.
+        reads through one bf16 staging pool shared by all layers; so does the mixed mode, for its chunks.
 
         CUDA bf16 models with head size 64, 80 or 128 run the flash / paged decode / paged prefill / append kernels;
         otherwise (CPU, fp32, other head sizes) their PyTorch references run, over FP8 pools too (append: not over FP8
@@ -761,6 +769,20 @@ class BloomForCausalLM(nn.Module):
             if seg_start is not None:
                 write(qkv, slot, k_pools[li], v_pools[li], D, **scales)
                 return A.alibi_attention(qkv, slopes, 1, N, n_head, D, seg_start=seg_start.view(1, N)).view(1, N, -1)
+            if n_dec is not None:
+                dec, new = qkv[:n_dec], qkv[n_dec:]
+                write(new, slot, k_pools[li], v_pools[li], D, **scales)
+                chunk = dict(scales, stage=staging) if staging is not None else scales
+                args = (new, k_pools[li], v_pools[li], table[n_dec:], cu_seqlens, start, max_len, slopes, D)
+                dec_args = (dec, k_pools[li], v_pools[li], table[:n_dec], positions[:n_dec], max_pos, slopes, D)
+                if not native:                                   # the references
+                    out = prefill(*args, **chunk)
+                    return (torch.cat([decode(*dec_args, **scales), out]) if n_dec else out).view(1, N, -1)
+                out = qkv.new_empty(N, n_head * D)               # both kernels write their rows of one buffer
+                prefill(*args, out=out[n_dec:], **chunk)
+                if n_dec:
+                    decode(*dec_args, out=out[:n_dec], **scales)
+                return out.view(1, N, -1)
             if start is not None:
                 write(qkv, slot, k_pools[li], v_pools[li], D, **scales)
                 if staging is not None:
@@ -773,7 +795,7 @@ class BloomForCausalLM(nn.Module):
             return decode(qkv, k_pools[li], v_pools[li], table, positions, max_pos, slopes, D, **scales).view(1, N, -1)
 
         x = self._inference_layers(self._inference_embed(ids.view(1, N), pos_emb), attend)[0]
-        return self._inference_head(x if seg_start is None and start is None else x[last.long()])
+        return self._inference_head(x if last is None else x[last.long()])
 
     def _incremental_logits_tp(self, ids: torch.Tensor, cache: list, past: int,
                                lead: Optional[torch.Tensor] = None, capacity: Optional[int] = None) -> torch.Tensor:

@@ -12,7 +12,8 @@ until it finishes, so nothing is ever preempted, and return to the free list in 
 
 A step is either one prefill of newly admitted prompts, packed into one row of at most ``max_prefill_tokens`` tokens
 (a longer prompt runs alone) through the document-masked flash kernel, or one decode of every running sequence
-through the paged split-KV decode kernel (or, with speculative decoding, a verify step: below).  Tokens are chosen with the model's ``_select_token``, one call per group of
+through the paged split-KV decode kernel (or, with speculative decoding, a verify step; with chunked prefill, a mixed
+step: below).  Tokens are chosen with the model's ``_select_token``, one call per group of
 requests that share sampling parameters.  A step makes one host-to-device upload (tokens, positions and page tables,
 shared by all layers) and one device-to-host transfer (the chosen tokens).
 
@@ -39,6 +40,20 @@ flash kernel runs on ``qkv``; only the cache write quantizes), and a decode step
 prefill with hits dequantizes the sequences' cached pages into a bf16 staging pool sized for the step's prompt pages
 and runs the paged prefill kernel on it.  A scale belongs to its page slot, so prefix sharing, reference counting and
 eviction are unchanged.  Accuracy on trained checkpoints is not verified here.
+
+Chunked prefill (``chunked_prefill=True``, off by default): a step then carries one decode token of every running
+request and, after them, chunks of admitted prompts, taken first come, first served until the step holds
+``max_prefill_tokens`` prompt tokens (decode tokens do not count).  A chunk that does not end its prompt ends on a page
+boundary, so every chunk starts on one (a prefix-cache start is one too), and the rest of that prompt waits for the
+next step; ``max_prefill_tokens`` must be at least 64.  The decode rows go through the paged decode kernel and the
+chunks through the paged prefill kernel over the pools (over FP8 pools through a staging pool of the chunks' pages, as
+a prefill with hits), in one forward; they write disjoint pages.  A request whose
+prompt completes chooses its first token in that step and decodes from the next; only then are its pages indexed and
+its ``cached`` counted in ``cached_prompt_tokens``.  A step without admitted prompts is the decode step above, and a step
+without running requests carries only chunks.  So a long prompt delays the running requests by one bounded step at a
+time instead of its whole prefill.  With FP8 pools a chunk reads the earlier chunks of its prompt from the pools,
+dequantized (positions computed in earlier steps), so a chunked prompt's logits differ from those of an unchunked
+prefill by the FP8 rounding of those keys and values.  Refused with speculative decoding.
 
 Speculative decoding (``num_speculative_tokens=k``, 0 .. 7, off by default; refused with FP8 pools): before a decode
 step every running request drafts up to k tokens by prompt lookup, the tokens that followed the most recent earlier
@@ -114,6 +129,7 @@ class _Request:
     eos_token_id: Optional[int]
     pages: List[int] = field(default_factory=list)
     cached: int = 0            # prompt positions served from the prefix cache (a multiple of the page size)
+    filled: int = 0            # chunked prefill: prompt positions in the cache so far (at least ``cached``)
     ngrams: Optional[_NgramIndex] = None      # speculative decoding only
 
     @property
@@ -132,11 +148,15 @@ class ContinuousBatcher:
     ``kv_cache_dtype``: ``None`` keeps the pools in the model's dtype, ``torch.float8_e4m3fn`` stores them in FP8 with
     per-position scales (module docstring).
     ``num_speculative_tokens``: most prompt-lookup drafts per request and decode step, 0 .. 7 (module docstring); 0
-    turns speculation off."""
+    turns speculation off.
+    ``chunked_prefill``: run prompts in page-aligned chunks of at most ``max_prefill_tokens`` tokens per step, in the
+    same steps as the running requests' decode tokens (module docstring); needs ``max_prefill_tokens >= 64`` and no
+    speculative decoding."""
 
     def __init__(self, model, max_cache_tokens: int, max_prefill_tokens: int = 8192,
                  generator: Optional[torch.Generator] = None, prefix_caching: bool = False,
-                 kv_cache_dtype: Optional[torch.dtype] = None, num_speculative_tokens: int = 0):
+                 kv_cache_dtype: Optional[torch.dtype] = None, num_speculative_tokens: int = 0,
+                 chunked_prefill: bool = False):
         from pipegoose_b200.models.bloom import BloomMLP, _decodes_incrementally
 
         if getattr(model, "tp", None) is not None:
@@ -157,6 +177,12 @@ class ContinuousBatcher:
                              f"{num_speculative_tokens}")
         if num_speculative_tokens and kv_cache_dtype is not None:
             raise ValueError("speculative decoding does not support FP8 KV-cache pools")
+        if chunked_prefill and max_prefill_tokens < PAGE_SIZE:
+            raise ValueError(f"chunked prefill cuts prompts at page boundaries: max_prefill_tokens must be at least "
+                             f"{PAGE_SIZE}, got {max_prefill_tokens}")
+        if chunked_prefill and num_speculative_tokens:
+            raise ValueError("chunked prefill does not support speculative decoding")
+        self.chunked_prefill = bool(chunked_prefill)
         self.num_speculative_tokens = int(num_speculative_tokens)
         self.speculative_proposed_tokens = 0                      # drafts verified
         self.speculative_accepted_tokens = 0                      # accepted drafts emitted
@@ -190,7 +216,7 @@ class ContinuousBatcher:
             self._key_ids = itertools.count()
         self._ids = itertools.count()
         self._waiting: collections.deque = collections.deque()    # submitted, no pages yet
-        self._admitted: collections.deque = collections.deque()   # pages reserved, prompt not yet run
+        self._admitted: collections.deque = collections.deque()   # pages reserved, prompt not yet (wholly) run
         self._running: List[_Request] = []                        # prompt in the cache, decoding
 
     # ------------------------------------------------------------------ public
@@ -219,7 +245,8 @@ class ContinuousBatcher:
         return bool(self._waiting or self._admitted or self._running)
 
     def step(self) -> List[Tuple[int, List[int]]]:
-        """One prefill or one decode step; returns ``(rid, prompt + new tokens)`` of the requests that finished."""
+        """One prefill, decode or (chunked prefill) mixed step; returns ``(rid, prompt + new tokens)`` of the requests
+        that finished."""
         self._admit()
         spec = self._speculate() if self.num_speculative_tokens and not self._admitted else None
         if spec is not None:
@@ -335,6 +362,8 @@ class ContinuousBatcher:
     def _forward(self) -> Tuple[List[_Request], torch.Tensor]:
         """The requests this step serves, with requests that share sampling parameters adjacent, and their fp32
         next-token logits ``[len(reqs), V]``."""
+        if self._admitted and self.chunked_prefill:
+            return self._mixed()
         if self._admitted:                                      # prefill the oldest admitted prompts
             reqs, n = [], 0
             while self._admitted and (not reqs or n + self._admitted[0].prompt_len - self._admitted[0].cached
@@ -393,18 +422,78 @@ class ContinuousBatcher:
             start.append(st)
             table += r.pages + [0] * (width - len(r.pages))
         max_len = max(r.prompt_len - r.cached for r in reqs)
-        rows, stage = [ids, positions, slot, last, cu, start, table], None
-        if self.k_scales is not None:
-            n, src, dst, st_slot, st_table = fp8_prefill_staging([r.pages for r in reqs], [r.cached for r in reqs],
-                                                                 [r.prompt_len for r in reqs])
-            rows += [src, dst, st_slot, [p for row in st_table for p in row]]
-        up = self._upload(rows)
+        n, plan = self._staging([r.pages for r in reqs], [r.cached for r in reqs], [r.prompt_len for r in reqs])
+        up = self._upload([ids, positions, slot, last, cu, start, table] + plan)
         ids, positions, slot, last, cu, start, table = up[:7]
-        if self.k_scales is not None:
-            stage = (n, up[7], up[8], up[9], up[10].view(len(reqs), -1))
+        stage = (n, up[7], up[8], up[9], up[10].view(len(reqs), -1)) if plan else None
         return self.model._paged_logits(ids, positions, self.k_pools, self.v_pools, slot=slot, last=last,
                                         table=table.view(len(reqs), width), cu_seqlens=cu, start=start,
                                         max_len=max_len, k_scales=self.k_scales, v_scales=self.v_scales, stage=stage)
+
+    def _staging(self, pages: List[List[int]], starts: List[int], ends: List[int]) -> Tuple[int, List[List[int]]]:
+        """FP8 pools: the staging plan (:func:`fp8_prefill_staging`) of a prefill whose sequences have ``starts``
+        positions in the pools and ``ends`` in all, as its pool size and host rows for the step's upload; ``(0, [])``
+        with other pools."""
+        if self.k_scales is None:
+            return 0, []
+        n, src, dst, slot, table = fp8_prefill_staging(pages, starts, ends)
+        return n, [src, dst, slot, [p for row in table for p in row]]
+
+    def _chunks(self) -> List[Tuple[_Request, int, int]]:
+        """The step's prompt chunks ``(request, first position, end)``, first come, first served, at most
+        ``max_prefill_tokens`` tokens in all.  A chunk that does not end its prompt ends on a page boundary, and no
+        later request gets a chunk in that step."""
+        chunks, n = [], 0
+        for r in self._admitted:
+            s = max(r.filled, r.cached)
+            room = self.max_prefill_tokens - n
+            e = r.prompt_len if r.prompt_len - s <= room else (s + room) // PAGE_SIZE * PAGE_SIZE
+            if e > s:
+                chunks.append((r, s, e))
+                n += e - s
+            if e < r.prompt_len:
+                break
+        return chunks
+
+    def _mixed(self) -> Tuple[List[_Request], torch.Tensor]:
+        """Chunked prefill: one decode token of every running request, then the step's prompt chunks, through one
+        forward.  Requests whose prompt completes choose their first token in this step; the others stay admitted."""
+        dec = self._running
+        self._running = []
+        chunks = self._chunks()
+        width = max(len(r.pages) for r in dec + [c[0] for c in chunks])
+        ids = [r.tokens[-1] for r in dec]
+        positions = [len(r.tokens) - 1 for r in dec]
+        table = [p for r in dec + [c[0] for c in chunks] for p in r.pages + [0] * (width - len(r.pages))]
+        slot, cu, start, done, rows = [], [0], [], [], list(range(len(dec)))
+        for r, s, e in chunks:
+            ids += r.tokens[s:e]
+            positions += range(s, e)
+            slot += [r.pages[p // PAGE_SIZE] * PAGE_SIZE + p % PAGE_SIZE for p in range(s, e)]
+            cu.append(cu[-1] + e - s)
+            start.append(s)
+            r.filled = e
+            if e == r.prompt_len:
+                done.append(r)
+                rows.append(len(dec) + cu[-1] - 1)
+        for r in done:                                          # the oldest admitted requests
+            self._admitted.popleft()
+            if self.prefix_caching:
+                self.cached_prompt_tokens += r.cached
+                self._register(r, r.prompt_len)
+        reqs = dec + done
+        order = sorted(range(len(reqs)), key=lambda i: reqs[i].sampling)      # stable: groups of equal sampling
+        last = [rows[i] for i in order]
+        n, plan = self._staging([r.pages for r, _, _ in chunks], start, [e for _, _, e in chunks])
+        up = self._upload([ids, positions, table, slot, cu, start, last] + plan)
+        ids, positions, table, slot, cu, start, last = up[:7]
+        stage = (n, up[7], up[8], up[9], up[10].view(len(chunks), -1)) if plan else None
+        logits = self.model._paged_logits(ids, positions, self.k_pools, self.v_pools, slot=slot, last=last,
+                                          table=table.view(-1, width), max_pos=max([0] + [len(r.tokens) - 1 for r in dec]),
+                                          cu_seqlens=cu, start=start, max_len=max(e - s for _, s, e in chunks),
+                                          k_scales=self.k_scales, v_scales=self.v_scales, stage=stage,
+                                          n_dec=len(dec))
+        return [reqs[i] for i in order], logits.float()
 
     def _select(self, reqs: List[_Request], logits: torch.Tensor) -> List[int]:
         """Next token of every request (``reqs`` grouped by sampling parameters), one device-to-host transfer."""
