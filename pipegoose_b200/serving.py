@@ -70,6 +70,24 @@ values behind the accepted ones; the next step of that request writes those posi
 and ``_release`` indexes only the valid positions.  ``speculative_proposed_tokens`` counts the drafts verified and
 ``speculative_accepted_tokens`` the accepted drafts that were emitted (not those cut off after an eos).
 
+CUDA graphs (``cuda_graphs=True``, off by default): the plain decode step (one token per running request through the
+paged decode kernel, in every mode above: the decode steps of the default engine, steps without chunks under chunked
+prefill, steps without drafts under speculative decoding, and over FP8 pools) is replayed from a CUDA graph instead of
+being issued op by op from Python.  Prefill steps (with or without cached prefixes), mixed steps and verify steps stay
+eager.  A step with B running requests replays the graph of the smallest of ``GRAPH_BATCH_SIZES`` that holds B; a
+larger step runs eager.  A bucket's graph is captured on the first step that needs it (after one eager warm-up call
+on the capture stream) and kept for the engine's lifetime; all graphs share one memory pool.  Every graph reads one
+static int32 buffer (ids, positions, and page tables of one width W, the most pages one request can reserve), filled
+from a pinned host mirror by one copy per step, and is captured with ``max_pos = W * 64 - 1``, which only shapes the
+kernel's grid.  Rows past B are padding: token 0 at position 0 over a table row of the scratch page, one extra page
+(index ``num_pages``) of every pool and scale pool that never enters the free list.  The graph writes the logits into
+a static ``[bucket, V]`` buffer and token choice runs eagerly on its first B rows, so it is the eager engine's choice
+for the same logits.  A bucket's kernel grid, and cuBLAS's choice for the padded M, can differ from the eager step's,
+so logits can differ from the eager engine's at rounding level.  Costs: the graphs' pool (the largest bucket's logits
+alone are 256 x V model-dtype values) and a capture pause the first time a bucket is used.  Needs the native decode
+path (CUDA bf16 weights, head size 64, 80 or 128) and ``BloomMLP`` MLPs (``ExpertLayer`` routing depends on the data):
+refused otherwise.  ``graph_decode_steps`` counts the decode steps served by a replay.
+
 Limits: sampled tokens depend on which requests share a step (the random stream is consumed per group; in a verify
 step a group takes one uniform number per token row, then one draw per row without the draft, then one per row);
 an ``ExpertLayer`` capacity limit counts the tokens of one step, as in ``generate()`` (with prefix caching, cached keys
@@ -89,6 +107,7 @@ from pipegoose_b200.ops.attention import APPEND_MAX_TOKENS, PAGE_SIZE, fp8_prefi
 
 SPEC_NGRAM_SIZES = (3, 2)                           # trailing n-gram sizes the drafter looks up, longest first
 MAX_SPECULATIVE_TOKENS = APPEND_MAX_TOKENS - 1      # drafts per request and step: with the last token, one append
+GRAPH_BATCH_SIZES = (1, 2, 4, 8, 16, 32, 64, 128, 256)   # decode batch buckets captured as CUDA graphs (cuda_graphs)
 
 
 class _NgramIndex:
@@ -151,13 +170,16 @@ class ContinuousBatcher:
     turns speculation off.
     ``chunked_prefill``: run prompts in page-aligned chunks of at most ``max_prefill_tokens`` tokens per step, in the
     same steps as the running requests' decode tokens (module docstring); needs ``max_prefill_tokens >= 64`` and no
-    speculative decoding."""
+    speculative decoding.
+    ``cuda_graphs``: replay plain decode steps of at most ``GRAPH_BATCH_SIZES[-1]`` requests from CUDA graphs, one per
+    batch bucket, captured on first use (module docstring); costs the graphs' memory pool and one capture pause per
+    bucket.  Needs a model on the native decode path with ``BloomMLP`` MLPs."""
 
     def __init__(self, model, max_cache_tokens: int, max_prefill_tokens: int = 8192,
                  generator: Optional[torch.Generator] = None, prefix_caching: bool = False,
                  kv_cache_dtype: Optional[torch.dtype] = None, num_speculative_tokens: int = 0,
-                 chunked_prefill: bool = False):
-        from pipegoose_b200.models.bloom import BloomMLP, _decodes_incrementally
+                 chunked_prefill: bool = False, cuda_graphs: bool = False):
+        from pipegoose_b200.models.bloom import BloomMLP, _decodes_incrementally, _native_decode
 
         if getattr(model, "tp", None) is not None:
             raise ValueError("ContinuousBatcher serves single-GPU models: tensor-parallel models are not supported")
@@ -182,6 +204,16 @@ class ContinuousBatcher:
                              f"{PAGE_SIZE}, got {max_prefill_tokens}")
         if chunked_prefill and num_speculative_tokens:
             raise ValueError("chunked prefill does not support speculative decoding")
+        w = blocks[0].self_attention.query_key_value.weight
+        D = model.config.hidden_size // model.config.n_head
+        if cuda_graphs and not all(isinstance(b.mlp, BloomMLP) for b in blocks):
+            raise ValueError("cuda_graphs needs BloomMLP MLPs: ExpertLayer routing depends on the data, so its decode "
+                             "step cannot be captured")
+        if cuda_graphs and not _native_decode(w, D):
+            raise ValueError("cuda_graphs needs the native decode path: CUDA bf16 weights and a head size of 64, 80 or "
+                             f"128 (got {w.dtype} on {w.device}, head size {D})")
+        self.cuda_graphs = bool(cuda_graphs)
+        self.graph_decode_steps = 0                               # decode steps served by a graph replay
         self.chunked_prefill = bool(chunked_prefill)
         self.num_speculative_tokens = int(num_speculative_tokens)
         self.speculative_proposed_tokens = 0                      # drafts verified
@@ -194,9 +226,8 @@ class ContinuousBatcher:
         if self.num_pages < 1:
             raise ValueError(f"max_cache_tokens = {max_cache_tokens} holds no page of {PAGE_SIZE} positions")
         self.n_positions = cfg.n_positions if getattr(cfg, "position_embedding", "alibi") == "learned" else None
-        w = blocks[0].self_attention.query_key_value.weight
-        D = cfg.hidden_size // cfg.n_head
-        shape = (len(blocks), self.num_pages, cfg.n_head, PAGE_SIZE, D)
+        # with cuda_graphs, one more page (index num_pages) that only the graphs' padding rows write
+        shape = (len(blocks), self.num_pages + self.cuda_graphs, cfg.n_head, PAGE_SIZE, D)
         self.k_pools = torch.empty(shape, dtype=kv_cache_dtype or w.dtype, device=w.device)
         self.v_pools = torch.empty(shape, dtype=kv_cache_dtype or w.dtype, device=w.device)
         self.k_scales = self.v_scales = None
@@ -218,6 +249,8 @@ class ContinuousBatcher:
         self._waiting: collections.deque = collections.deque()    # submitted, no pages yet
         self._admitted: collections.deque = collections.deque()   # pages reserved, prompt not yet (wholly) run
         self._running: List[_Request] = []                        # prompt in the cache, decoding
+        if self.cuda_graphs:
+            self._init_graphs()
 
     # ------------------------------------------------------------------ public
     def submit(self, prompt_ids: Sequence[int], max_new_tokens: int, do_sample: bool = False, temperature: float = 1.0,
@@ -382,6 +415,8 @@ class ContinuousBatcher:
         self._running = []
         if not reqs:
             return [], None
+        if self.cuda_graphs and len(reqs) <= self._graph_sizes[-1]:
+            return reqs, self._graph_decode(reqs).float()
         width = max(len(r.pages) for r in reqs)
         table = [p for r in reqs for p in r.pages + [0] * (width - len(r.pages))]
         pos = [len(r.tokens) - 1 for r in reqs]
@@ -494,6 +529,80 @@ class ContinuousBatcher:
                                           k_scales=self.k_scales, v_scales=self.v_scales, stage=stage,
                                           n_dec=len(dec))
         return [reqs[i] for i in order], logits.float()
+
+    # ------------------------------------------------------------------ CUDA graphs
+    def _init_graphs(self) -> None:
+        """The decode graphs' static inputs: one int32 device buffer and its pinned host mirror.  Bucket n uses the
+        prefix ``ids [n] | positions [n] | table [n, W]``, W the most pages one request can reserve."""
+        self._graph_sizes = tuple(sorted(GRAPH_BATCH_SIZES))
+        self._graph_width = self.num_pages
+        if self.n_positions is not None:            # a request holds at most n_positions + 1 positions (submit)
+            self._graph_width = min(self.num_pages, -(-(self.n_positions + 1) // PAGE_SIZE))
+        size = self._graph_sizes[-1] * (2 + self._graph_width)
+        self._graph_in = torch.zeros(size, dtype=torch.int32, device=self.device)
+        self._graph_host = torch.zeros(size, dtype=torch.int32).pin_memory()
+        self._graphs: Dict[int, Tuple] = {}                         # bucket -> (graph, static logits, decode tickets)
+        self._graph_pool = torch.cuda.graph_pool_handle()
+        self._graph_stream = torch.cuda.Stream(self.device)
+
+    def _graph_inputs(self, n: int, ids: List[int], positions: List[int],
+                      pages: List[List[int]]) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Fill bucket ``n``'s static inputs, in one host-to-device copy: the ``len(ids)`` rows given, then padding rows
+        (token 0 at position 0, a table row of the scratch page ``num_pages``); returns the device views ``ids [n]``,
+        ``positions [n]`` and ``table [n, W]``.  Table entries behind a row's pages keep older values: the kernel reads
+        only the pages of positions ``0 .. positions[b]``.
+
+        Invariant: padding rows write their key and value into slot 0 of the scratch page and read only that key, from
+        their own qkv row (the decode kernel takes the key at ``positions[b]`` from qkv), so no real row ever reads the
+        scratch page and the padding rows' concurrent writes to it are harmless."""
+        W, B, scratch = self._graph_width, len(ids), self.num_pages
+        host = self._graph_host[:n * (2 + W)]
+        host[:2 * n] = torch.tensor(ids + [0] * (n - B) + positions + [0] * (n - B), dtype=torch.int32)
+        table = host[2 * n:].view(n, W)
+        if B:
+            w = max(len(p) for p in pages)
+            table[:B, :w] = torch.tensor([p + [scratch] * (w - len(p)) for p in pages], dtype=torch.int32)
+        table[B:] = scratch
+        dev = self._graph_in[:host.numel()]
+        dev.copy_(host, non_blocking=True)
+        return dev[:n], dev[n:2 * n], dev[2 * n:].view(n, W)
+
+    def _graph_call(self, ids: torch.Tensor, positions: torch.Tensor, table: torch.Tensor) -> torch.Tensor:
+        """The decode forward a graph holds, on static inputs: logits ``[n, V]`` in the model's dtype."""
+        return self.model._paged_logits(ids, positions, self.k_pools, self.v_pools, table=table,
+                                        max_pos=self._graph_width * PAGE_SIZE - 1, k_scales=self.k_scales,
+                                        v_scales=self.v_scales)
+
+    def _graph(self, n: int) -> Tuple:
+        """Bucket ``n``'s ``(graph, static logits [n, V], decode tickets)``, captured on first use.  Warm-up and capture
+        run on all-padding inputs, so they write only the scratch page while the pools hold live requests."""
+        from pipegoose_b200.ops.attention import _decode_ticket
+
+        if n in self._graphs:
+            return self._graphs[n]
+        inputs = self._graph_inputs(n, [], [], [])
+        s = self._graph_stream
+        s.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(s):
+            # one eager call first: the decode-ticket array (zero-filled), the ALiBi slope caches and cuBLAS's handle
+            # and workspace are made on first use, and a capture would only record their initialisation
+            self._graph_call(*inputs)
+        s.synchronize()                                   # the host mirror is refilled before the replay
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, pool=self._graph_pool, stream=s):
+            logits = self._graph_call(*inputs)
+        # the graph keeps using the ticket array it captured: hold it, since a larger eager step replaces the cached one
+        self._graphs[n] = (graph, logits, _decode_ticket(0, self.device))
+        return self._graphs[n]
+
+    def _graph_decode(self, reqs: List[_Request]) -> torch.Tensor:
+        """The plain decode step by graph replay: logits ``[len(reqs), V]``, the first rows of the bucket's."""
+        n = next(s for s in self._graph_sizes if s >= len(reqs))
+        graph, logits, _ = self._graph(n)
+        self._graph_inputs(n, [r.tokens[-1] for r in reqs], [len(r.tokens) - 1 for r in reqs], [r.pages for r in reqs])
+        graph.replay()
+        self.graph_decode_steps += 1
+        return logits[:len(reqs)]
 
     def _select(self, reqs: List[_Request], logits: torch.Tensor) -> List[int]:
         """Next token of every request (``reqs`` grouped by sampling parameters), one device-to-host transfer."""
