@@ -33,26 +33,13 @@
 // position may hold anything (NaN included): the second page of the last block is not loaded when it lies wholly
 // past it, and V rows past it are zeroed in shared memory before P.V (a masked p = 0 times NaN would still be NaN).
 // D = 80 runs as D = 128: the pool maps have 80 columns, so TMA's out-of-bounds fill zeroes K / V columns 80..127.
-//
-// Paged prefill over FP8 pools (PAGED and FP8): the same CTA, consumer loop and output, but the K / V tiles are built by
-// the whole producer warpgroup instead of TMA.  Every start[r] is a multiple of 64, so each page of a block is either
-// wholly cached (before start[r]: e4m3 codes and per-position scales read from the pools and converted to bf16 with
-// the arithmetic of kv_dequantize_kernel, bf16(float(code) * scale)) or wholly new (the step's own tokens: their
-// keys and values read from qkv rows cu_seqlens[r] + p - start[r], exactly).  The threads store 16-byte chunks into
-// the 128B-swizzled slots the TMA boxes would have filled, fence them to the async proxy and arrive on kv_full (128
-// arrivals, no transaction bytes).  No new token past the CTA's last query is read; D = 80 stores zeros in columns
-// 80..127.  The producer warpgroup keeps 24 registers per thread: the CTA holds 168 * 384 registers, so the consumers'
-// 240 leave no more (a 32-register producer would leave setmaxnreg.inc waiting forever); with one load in flight per
-// thread the fill has 0 spill bytes.
 #include "launch.h"
 #include "pdl_launch.cuh"
 #include "ptx.cuh"
 #include "wgmma.cuh"
-#include <cuda_fp8.h>
 #include <cstdio>
 #include <cstring>
 #include <mutex>
-#include <type_traits>
 #include <unordered_map>
 
 namespace pg {
@@ -107,71 +94,10 @@ struct AttFwdArgs {
   int d_out;              // columns stored per head (80 for bloom-3b on the D = 128 instantiation)
 };
 
-// PAGED over FP8 pools: the kernel's K / V parameters in place of the pool tensor maps (the tensor maps would come
-// after AttFwdArgs in the parameter list, so new AttFwdArgs fields would move them in the other instantiations)
-struct PagedFp8Pool {
-  const uint8_t* codes;      // [num_pages, H_pool, 64, d_out] e4m3
-  const float* scales;       // [num_pages, H_pool, 64]
-  const __nv_bfloat16* qkv;  // column of this part (K or V) of head 0 in qkv [N, H * 3 * d_out]: the new tokens
-};
-
-// 16 e4m3 codes times their row's scale -> 16 bf16, as kv_dequantize_kernel computes them
-PG_DEVICE void dequant_fp8x16(const uint4& c, float sc, uint4& y0, uint4& y1) {
-  const __nv_fp8x2_storage_t* p = reinterpret_cast<const __nv_fp8x2_storage_t*>(&c);
-  uint32_t w[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float2 f = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2(p[i], __NV_E4M3)));
-    const __nv_bfloat162 b = __floats2bfloat162_rn(f.x * sc, f.y * sc);
-    w[i] = *reinterpret_cast<const uint32_t*>(&b);
-  }
-  y0 = make_uint4(w[0], w[1], w[2], w[3]);
-  y1 = make_uint4(w[4], w[5], w[6], w[7]);
-}
-
-// 16-byte chunk c (8 bf16 columns) of row r of a [128 rows x D] tile: D/64 atoms of [128 rows x 128 B], 128B swizzle
-PG_DEVICE uint8_t* tile_chunk(uint8_t* tile, int r, int c) {
-  return tile + (c >> 3) * 16384 + r * 128 + (((c & 7) ^ (r & 7)) << 4);
-}
-
-// PAGED over FP8 pools: page pg (64 keys from position p0) of a stage's K and V tiles, by the 128 producer threads t.
-// A cached page is read from the pools at pool row prow (page * H + head) * 64; a new page from qkv row n_first.
-template <int D>
-PG_DEVICE void fill_page_fp8(const AttFwdArgs& args, const PagedFp8Pool& pk, const PagedFp8Pool& pv, uint8_t* tk,
-                             uint8_t* tv, int pg, int t, bool cached, size_t prow, int n_first, int rows, int head) {
-  if (cached) {
-    constexpr int W = D / 16;                 // 16-column units of a row
-    for (int i = t; i < 2 * 64 * W; i += 128) {
-      const int kv = i / (64 * W), r = (i / W) % 64, u = i % W;
-      uint4 y0 = make_uint4(0, 0, 0, 0), y1 = y0;
-      if (16 * u < args.d_out) {
-        const PagedFp8Pool& pool = kv ? pv : pk;
-        const size_t row = prow + r;
-        dequant_fp8x16(ld_global_nc_v4(pool.codes + row * args.d_out + 16 * u), __ldg(pool.scales + row), y0, y1);
-      }
-      *reinterpret_cast<uint4*>(tile_chunk(kv ? tv : tk, 64 * pg + r, 2 * u)) = y0;
-      *reinterpret_cast<uint4*>(tile_chunk(kv ? tv : tk, 64 * pg + r, 2 * u + 1)) = y1;
-    }
-  } else {
-    constexpr int W = D / 8;                  // 8-column chunks of a row
-    const int ld = args.H * 3 * args.d_out;
-    const size_t src = static_cast<size_t>(n_first) * ld + head * 3 * args.d_out;
-    for (int i = t; i < 2 * 64 * W; i += 128) {
-      const int kv = i / (64 * W), r = (i / W) % 64, u = i % W;
-      if (r >= rows) continue;                // past the CTA's last query: never read
-      uint4 x = make_uint4(0, 0, 0, 0);
-      if (8 * u < args.d_out) x = ld_global_nc_v4((kv ? pv : pk).qkv + src + static_cast<size_t>(r) * ld + 8 * u);
-      *reinterpret_cast<uint4*>(tile_chunk(kv ? tv : tk, 64 * pg + r, u)) = x;
-    }
-  }
-}
-
-template <int D, bool SEG, bool PAGED = false, bool FP8 = false,
-          typename KV = std::conditional_t<FP8, PagedFp8Pool, CUtensorMap>>
+template <int D, bool SEG, bool PAGED = false>
 __global__ void __launch_bounds__(kAttThreads, 1)
     attention_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const AttFwdArgs args,
-                         const __grid_constant__ KV tm_k, const __grid_constant__ KV tm_v) {
-  static_assert(!FP8 || (PAGED && !SEG), "FP8 pools: paged prefill only");
+                         const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v) {
   using Cfg = AttFwdCfg<D>;
   constexpr int ST = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -196,13 +122,13 @@ __global__ void __launch_bounds__(kAttThreads, 1)
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tm_qkv);
-    if constexpr (PAGED && !FP8) {
+    if constexpr (PAGED) {
       tma_prefetch_desc(&tm_k);
       tma_prefetch_desc(&tm_v);
     }
     mbar_init(q_full, 1);
     for (int i = 0; i < ST; ++i) {
-      mbar_init(&kv_full[i], FP8 ? 128 : 1);  // FP8: one arrival per producer thread
+      mbar_init(&kv_full[i], 1);
       mbar_init(&kv_empty[i], 2);  // one arrival per consumer warpgroup
     }
     fence_mbar_init();
@@ -227,34 +153,7 @@ __global__ void __launch_bounds__(kAttThreads, 1)
 
   if (warp < 4) {
     setmaxnreg_dec<kAttRegsLight>();
-    if constexpr (FP8) {
-      // ===================== producer warpgroup: Q by TMA, K / V tiles built by all 128 threads =====================
-      if (warp == 0 && lane == 0) {
-        mbar_arrive_expect_tx(q_full, Cfg::kTileBytes);
-#pragma unroll
-        for (int a = 0; a < D / 64; ++a) tma_load_2d(sQ + a * 16384, &tm_qkv, q_full, col_q + a * 64, row0);
-      }
-      const int n0 = args.cu_seqlens[batch], st = args.start[batch];
-      const int* trow = args.table + static_cast<size_t>(batch) * args.max_pages;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int j = j0; j < num_kb; ++j) {
-        mbar_wait(&kv_empty[stage], phase ^ 1);
-        const int pages = j * ATT_BN + 64 <= p_last ? 2 : 1;
-        for (int pg = 0; pg < pages; ++pg) {
-          const int p0 = j * ATT_BN + 64 * pg;
-          fill_page_fp8<D>(args, tm_k, tm_v, sK + stage * Cfg::kTileBytes, sV + stage * Cfg::kTileBytes, pg, threadIdx.x,
-                           p0 < st, (static_cast<size_t>(trow[2 * j + pg]) * args.H_pool + head) * 64,
-                           n0 + p0 - st, min(64, p_last + 1 - p0), head);
-        }
-        fence_proxy_async_smem();  // generic-proxy tile stores -> wgmma reads
-        mbar_arrive(&kv_full[stage]);
-        if (++stage == ST) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    } else if (warp == 0) {
+    if (warp == 0) {
       // ===================== TMA producer =====================
       if (lane == 0) {
         mbar_arrive_expect_tx(q_full, Cfg::kTileBytes);
@@ -936,53 +835,6 @@ extern "C" int pg_paged_prefill_attention(const void* qkv, const void* k_pool, c
   a.H_pool = H;
   a.d_out = D;
   return D == 64 ? launch_att_fwd_paged<64>(tq, tk, tv, a, s) : launch_att_fwd_paged<128>(tq, tk, tv, a, s);
-}
-
-template <int D>
-static int launch_att_fwd_paged_fp8(const CUtensorMap& tq, const AttFwdArgs& a, const PagedFp8Pool& pk,
-                                    const PagedFp8Pool& pv, cudaStream_t s) {
-  using Cfg = AttFwdCfg<D>;
-  static bool set = false;
-  if (!set) {
-    if (cudaFuncSetAttribute(attention_fwd_kernel<D, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) != cudaSuccess) return -1;
-    set = true;
-  }
-  dim3 grid((a.S + ATT_BM - 1) / ATT_BM, a.H, a.B);
-  if (launch_pdl(attention_fwd_kernel<D, false, true, true>, grid, dim3(kAttThreads), Cfg::kSmemBytes, s, tq, a, pk, pv) != cudaSuccess)
-    return -1;
-  PG_CHECK_LAUNCH("attention_fwd_paged_fp8");
-  return 0;
-}
-
-// pg_paged_prefill_attention over FP8 pools (PAGED and FP8, see the top of the file): cached positions (before
-// start[r], a multiple of 64) are read from the e4m3 codes k_pool / v_pool [num_pages, H, 64, D] and fp32 scales
-// k_scales / v_scales [num_pages, H, 64]; the new tokens' keys and values from qkv, exactly.
-extern "C" int pg_paged_prefill_attention_fp8(const void* qkv, const void* k_pool, const void* v_pool,
-                                              const float* k_scales, const float* v_scales, const int* table,
-                                              const int* cu_seqlens, const int* start, const float* slopes, void* out,
-                                              int N, int R, int H, int D, int max_pages, int max_len,
-                                              float softmax_scale, cudaStream_t s) {
-  if (D != 64 && D != 80 && D != 128) return -1;
-  if (N <= 0 || R <= 0 || max_len <= 0) return 0;
-  CUtensorMap tq;
-  if (att_tmap(&tq, qkv, static_cast<uint64_t>(N), static_cast<uint64_t>(H) * 3 * D, ATT_BM) != 0) return -1;
-  AttFwdArgs a;
-  memset(&a, 0, sizeof(a));
-  a.out = (__nv_bfloat16*)out;
-  a.slopes = slopes;
-  a.B = R; a.S = max_len; a.H = H;
-  a.ld_out = H * D;
-  a.scale_log2 = kLog2e * (softmax_scale > 0.f ? softmax_scale : 1.0f / sqrtf(static_cast<float>(D)));
-  a.cu_seqlens = cu_seqlens;
-  a.start = start;
-  a.table = table;
-  a.max_pages = max_pages;
-  a.H_pool = H;
-  a.d_out = D;
-  const __nv_bfloat16* q = static_cast<const __nv_bfloat16*>(qkv);
-  const PagedFp8Pool pk{static_cast<const uint8_t*>(k_pool), k_scales, q + D};
-  const PagedFp8Pool pv{static_cast<const uint8_t*>(v_pool), v_scales, q + 2 * D};
-  return D == 64 ? launch_att_fwd_paged_fp8<64>(tq, a, pk, pv, s) : launch_att_fwd_paged_fp8<128>(tq, a, pk, pv, s);
 }
 
 template <int D, bool SEG>

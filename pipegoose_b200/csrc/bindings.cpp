@@ -714,43 +714,6 @@ void paged_decode_attention_fp8(const torch::Tensor& qkv, torch::Tensor k_pool, 
                                             cur_stream()) == 0, "paged_decode_attention_fp8 failed");
 }
 
-// paged_prefill_attention over FP8 pools: positions before start[r] (a multiple of 64, not checked here) are read from
-// the e4m3 pools with their scales, the new tokens' keys and values from qkv, exactly.
-void paged_prefill_attention_fp8(const torch::Tensor& qkv, const torch::Tensor& k_pool, const torch::Tensor& v_pool,
-                                 const torch::Tensor& k_scales, const torch::Tensor& v_scales,
-                                 const torch::Tensor& table, const torch::Tensor& cu_seqlens,
-                                 const torch::Tensor& start, int64_t max_len, const torch::Tensor& slopes,
-                                 torch::Tensor out, double softmax_scale) {
-  PG_CUDA(qkv); PG_BF16(qkv);
-  check_fp8_pools(k_pool, v_pool, k_scales, v_scales, qkv.device(), "paged_prefill_attention_fp8");
-  TORCH_CHECK(reinterpret_cast<uintptr_t>(qkv.data_ptr()) % 16 == 0, "paged_prefill_attention_fp8: qkv must be 16B aligned");
-  PG_CUDA(out); PG_BF16(out); PG_CUDA(slopes); PG_F32(slopes); PG_CUDA(table); PG_CUDA(cu_seqlens); PG_CUDA(start);
-  TORCH_CHECK(table.scalar_type() == torch::kInt32 && cu_seqlens.scalar_type() == torch::kInt32 &&
-              start.scalar_type() == torch::kInt32, "paged_prefill_attention_fp8: table, cu_seqlens and start must be int32");
-  TORCH_CHECK(table.dim() == 2 && table.size(1) >= 1 && table.is_contiguous(),
-              "paged_prefill_attention_fp8: table must be a contiguous [R, max_pages]");
-  const int64_t R = table.size(0), H = k_pool.size(1), D = k_pool.size(3), max_pages = table.size(1);
-  TORCH_CHECK(cu_seqlens.numel() == R + 1 && start.numel() == R && cu_seqlens.is_contiguous() && start.is_contiguous(),
-              "paged_prefill_attention_fp8: cu_seqlens must be [R+1] and start [R] for the R = ", R, " table rows");
-  TORCH_CHECK(qkv.dim() == 2 && qkv.size(1) == H * 3 * D && qkv.is_contiguous(),
-              "paged_prefill_attention_fp8: qkv must be a contiguous [N, H*3*D]");
-  const int64_t N = qkv.size(0);
-  TORCH_CHECK(out.numel() == N * H * D && out.is_contiguous() && slopes.numel() == H,
-              "paged_prefill_attention_fp8: shape mismatch");
-  TORCH_CHECK(1 <= max_len && max_len <= max_pages * 64, "paged_prefill_attention_fp8: max_len ", max_len,
-              " outside 1 .. the ", max_pages * 64, " positions of a table row");
-  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&out, &slopes, &table, &cu_seqlens, &start})
-    TORCH_CHECK(t->device() == qkv.device(), "paged_prefill_attention_fp8: tensors on different devices");
-  if (N == 0 || R == 0) return;
-  c10::cuda::CUDAGuard guard(qkv.device());
-  TORCH_CHECK(pg_paged_prefill_attention_fp8(qkv.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(),
-                                             k_scales.data_ptr<float>(), v_scales.data_ptr<float>(),
-                                             table.data_ptr<int>(), cu_seqlens.data_ptr<int>(), start.data_ptr<int>(),
-                                             slopes.data_ptr<float>(), out.data_ptr(), (int)N, (int)R, (int)H, (int)D,
-                                             (int)max_pages, (int)max_len, (float)softmax_scale, cur_stream()) == 0,
-              "paged_prefill_attention_fp8 failed");
-}
-
 // Pages src[i] (int32 [n]) of the FP8 pools, dequantized, into pages dst[i] of the bf16 pools k_out / v_out
 // [*, H, 64, D].  The caller guarantees that every id is a page of its pool.
 void paged_kv_dequantize(const torch::Tensor& k_pool, const torch::Tensor& v_pool, const torch::Tensor& k_scales,
@@ -967,9 +930,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("paged_prefill_attention", &paged_prefill_attention, py::arg("qkv"), py::arg("k_pool"), py::arg("v_pool"),
         py::arg("table"), py::arg("cu_seqlens"), py::arg("start"), py::arg("max_len"), py::arg("slopes"), py::arg("out"),
         py::arg("softmax_scale"));
-  m.def("paged_prefill_attention_fp8", &paged_prefill_attention_fp8, py::arg("qkv"), py::arg("k_pool"),
-        py::arg("v_pool"), py::arg("k_scales"), py::arg("v_scales"), py::arg("table"), py::arg("cu_seqlens"),
-        py::arg("start"), py::arg("max_len"), py::arg("slopes"), py::arg("out"), py::arg("softmax_scale"));
   m.def("paged_kv_write", &paged_kv_write, py::arg("qkv"), py::arg("slot"), py::arg("k_pool"), py::arg("v_pool"));
   m.def("paged_kv_write_fp8", &paged_kv_write_fp8, py::arg("qkv"), py::arg("slot"), py::arg("k_pool"),
         py::arg("v_pool"), py::arg("k_scales"), py::arg("v_scales"));

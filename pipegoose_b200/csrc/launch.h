@@ -100,14 +100,6 @@ int pg_paged_prefill_attention(const void* qkv, const void* k_pool, const void* 
                                const int* cu_seqlens, const int* start, const float* slopes, void* out, int N, int R,
                                int H, int D, int num_pages, int max_pages, int max_len, float softmax_scale,
                                cudaStream_t s);
-// The same over FP8 pools (e4m3 codes k_pool / v_pool [num_pages, H, 64, D], fp32 scales k_scales / v_scales
-// [num_pages, H, 64]): positions before start[r] (a multiple of 64) are read from the pools, dequantized to bf16 as
-// pg_paged_kv_dequantize does, and the new tokens' keys and values from qkv, exactly; the caller need not store them
-// first.
-int pg_paged_prefill_attention_fp8(const void* qkv, const void* k_pool, const void* v_pool, const float* k_scales,
-                                   const float* v_scales, const int* table, const int* cu_seqlens, const int* start,
-                                   const float* slopes, void* out, int N, int R, int H, int D, int max_pages,
-                                   int max_len, float softmax_scale, cudaStream_t s);
 
 // ---- decode_sm90.cu
 // One decoding step of B rows at column pos: writes the new k / v of qkv [B, H*3*D] into k_cache / v_cache
@@ -142,7 +134,8 @@ int pg_paged_kv_write(const void* qkv, const int* slot, void* k_pool, void* v_po
 // one per position and head (value = float(code) * scale).  pg_paged_kv_write_fp8 quantizes every token's k / v into
 // its slot.  pg_paged_decode_attention_fp8 is pg_paged_decode_attention over those pools: the key and value at pos[b]
 // come from qkv exactly and are quantized into their slot.  pg_paged_kv_dequantize writes pages src[i] (int32 [n]) of
-// the FP8 pools, dequantized to bf16, into pages dst[i] of k_out / v_out [*, H, 64, D].
+// the FP8 pools, dequantized to bf16, into pages dst[i] of k_out / v_out [*, H, 64, D]: the staging pool through which
+// pg_paged_prefill_attention reads a cached prefix held in FP8 pools.
 int pg_paged_kv_write_fp8(const void* qkv, const int* slot, void* k_pool, void* v_pool, float* k_scales,
                           float* v_scales, int N, int H, int D, cudaStream_t s);
 int pg_paged_decode_attention_fp8(const void* qkv, void* k_pool, void* v_pool, float* k_scales, float* v_scales,

@@ -735,7 +735,8 @@ class BloomForCausalLM(nn.Module):
         FP8 pools (``float8_e4m3fn``) come with fp32 ``k_scales`` / ``v_scales`` ``[n_layer, num_pages, n_head, 64]``;
         a prefill with cached prefixes then also takes ``stage = (num_pages, src, dst, slot, table)``, the device form of
         :func:`~pipegoose_b200.ops.attention.fp8_prefill_staging` (``table`` as ``[R, width]``), which the kernel path
-        reads through one bf16 staging pool shared by all layers; so does the mixed mode, for its chunks.
+        reads through one bf16 staging pool shared by all layers (the paged prefill op refuses FP8 pools without it);
+        so does the mixed mode, for its chunks.
 
         CUDA bf16 models with head size 64, 80 or 128 run the flash / paged decode / paged prefill / append kernels;
         otherwise (CPU, fp32, other head sizes) their PyTorch references run, over FP8 pools too (append: not over FP8
@@ -755,9 +756,7 @@ class BloomForCausalLM(nn.Module):
         # append: each sequence's first new position
         first = positions[cu_seqlens[:-1].long()] if cu_seqlens is not None and start is None else None
         staging = None
-        if native and k_scales is not None and start is not None:
-            if stage is None:
-                raise ValueError("a prefill with cached prefixes over FP8 pools needs its staging plan (stage)")
+        if native and k_scales is not None and stage is not None:
             shape = (stage[0], n_head, A.PAGE_SIZE, D)
             w = self.transformer.h[0].self_attention.query_key_value.weight
             staging = (w.new_empty(shape), w.new_empty(shape)) + tuple(stage[1:])

@@ -445,11 +445,8 @@ def paged_kv_dequantize(k_pool: torch.Tensor, v_pool: torch.Tensor, k_scales: to
 #
 # FP8 pools: the new tokens are read from ``qkv`` (the rule of the section above), the cached prefix from the pools.
 # Every ``start[r]`` is then a multiple of PAGE_SIZE (prefix caching shares full pages only, chunked prefill cuts
-# prompts at page boundaries).  The FP8 form of the kernel reads the cached pages' codes and scales and dequantizes
-# them in shared memory, and reads the new tokens' keys and values from ``qkv``; the pool write may come before or
-# after it.  The ``stage=`` form runs the bf16 kernel on a step-local staging pool that holds just the step's sequences
-# (:func:`fp8_prefill_staging`): their cached pages dequantized, then their new tokens' exact keys and values.  Both
-# compute the same bits.
+# prompts at page boundaries), so the kernel runs on a step-local bf16 staging pool that holds just the step's
+# sequences (:func:`fp8_prefill_staging`): their cached pages dequantized, then their new tokens' exact keys and values.
 # ---------------------------------------------------------------------------------------------------------------------
 
 def _check_prefill_bounds(cu_seqlens: torch.Tensor, max_len: int, table: torch.Tensor, D: int = 0) -> None:
@@ -619,30 +616,17 @@ def alibi_paged_prefill_attention(qkv: torch.Tensor, k_pool: torch.Tensor, v_poo
     ``[N, n_head*D]``.  CUDA bf16 inputs run the paged form of the flash kernel (``csrc/attention_sm90.cu``, D in
     64 / 80 / 128; D = 80 on the D = 128 instantiation without padded copies).
 
-    Over FP8 pools without ``stage`` the FP8 form of the kernel runs (every ``start[r]`` a multiple of PAGE_SIZE,
-    checked when ``start`` is a host tensor).  With ``stage = (k_stage, v_stage, src, dst, slot, table)`` the bf16
-    kernel reads a staging pool instead: the staging pools ``[>= num_pages, n_head, PAGE_SIZE, D]`` (their content is
-    overwritten) and the device int32 lists of :func:`fp8_prefill_staging` (``table`` as ``[R, width]``).  The two
-    give the same bits.  The reference path needs no ``stage``.  ``out`` (contiguous ``[N, n_head*D]``, kernel path
-    only) receives the result instead of a new tensor."""
+    Over FP8 pools the kernel reads a bf16 staging pool: ``stage = (k_stage, v_stage, src, dst, slot, table)``, the
+    staging pools ``[>= num_pages, n_head, PAGE_SIZE, D]`` (their content is overwritten) and the device int32 lists
+    of :func:`fp8_prefill_staging` (``table`` as ``[R, width]``).  The reference path needs no ``stage``.  ``out``
+    (contiguous ``[N, n_head*D]``, kernel path only) receives the result instead of a new tensor."""
     fp8 = _fp8_pools(k_pool, k_scales, v_scales)
     if not use_native(qkv):
         return alibi_paged_prefill_attention_reference(qkv, k_pool, v_pool, table, cu_seqlens, start, max_len, slopes,
                                                        D, softmax_scale, k_scales=k_scales, v_scales=v_scales)
-    if fp8 and stage is None:
-        _check_prefill_bounds(cu_seqlens, max_len, table, D)
-        if not start.is_cuda and bool((start % PAGE_SIZE != 0).any()):
-            raise ValueError(f"over FP8 pools every start must be a multiple of {PAGE_SIZE}, got {start.tolist()}")
-        n_head = k_pool.shape[1]
-        if out is None:
-            out = torch.empty(qkv.shape[0], n_head * D, dtype=qkv.dtype, device=qkv.device)
-        native().paged_prefill_attention_fp8(qkv.contiguous(), k_pool, v_pool, k_scales, v_scales,
-                                             table.to(torch.int32).contiguous(),
-                                             cu_seqlens.to(qkv.device, torch.int32).contiguous(),
-                                             start.to(qkv.device, torch.int32).contiguous(), int(max_len),
-                                             slopes.float().contiguous(), out, softmax_scale)
-        return out
     if fp8:
+        if stage is None:
+            raise ValueError("the paged prefill kernel reads FP8 pools through a staging pool: pass stage")
         k_stage, v_stage, src, dst, slot, table = stage
         paged_kv_dequantize(k_pool, v_pool, k_scales, v_scales, src, dst, k_stage, v_stage)
         paged_kv_write(qkv, slot, k_stage, v_stage, D)

@@ -1,13 +1,13 @@
-"""The eight attention kernels against one float64 reference, element by element, on inputs where every key counts.
+"""The attention kernels against one float64 reference, element by element, on inputs where every key counts.
 
 Every kernel computes the same thing: query i of head h sits at position p_i and sees keys lo_i <= k <= hi_i (hi_i =
 p_i) with the score ``q.k * scale + slope_h * (k - p_i)``.  :func:`attend` computes that in float64 from the values the
 kernel reads; thin adapters turn each layout (the flash kernels' fused ``[B*S, H*3*D]`` rows with ``seg_start``, the
 contiguous decode cache with ``lead``, the paged pools with their table, ``pos`` / ``cu_seqlens`` / ``start``) into
 that form.  Over FP8 pools the reference reads exactly what the kernel reads: ``float(code) * scale`` in the decode
-kernel, ``bf16(float(code) * scale)`` in the prefill kernel (``dequant_fp8x16``), and the step's own tokens exactly,
-from ``qkv``.  Quantization is an input to the reference, not part of the bound.  The backward reference is float64
-autograd through :func:`attend`.  The references run on the device in the GPU tests.
+kernel, ``bf16(float(code) * scale)`` in the prefill kernel's staging pool (``kv_dequantize_kernel``), and the step's
+own tokens exactly, from ``qkv``.  Quantization is an input to the reference, not part of the bound.  The backward
+reference is float64 autograd through :func:`attend`.  The references run on the device in the GPU tests.
 
 Bounds
 ------
@@ -79,8 +79,8 @@ from pipegoose_b200.ops import kernels as K
 from pipegoose_b200.ops.attention import (
     PAGE_SIZE, alibi_attention, alibi_attention_reference, alibi_decode_attention, alibi_decode_attention_reference,
     alibi_paged_append_attention, alibi_paged_append_attention_reference, alibi_paged_decode_attention,
-    alibi_paged_decode_attention_reference, alibi_paged_prefill_attention, pad_heads, padded_head_dim,
-    paged_prefill_attention_fp32, quantize_kv, unpad_heads)
+    alibi_paged_decode_attention_reference, alibi_paged_prefill_attention, fp8_prefill_staging, pad_heads,
+    padded_head_dim, paged_prefill_attention_fp32, quantize_kv, unpad_heads)
 
 gpu = pytest.mark.gpu
 
@@ -423,7 +423,7 @@ def _prefill_layout(regime, H, D, starts, news, fill, g, scale, fp8=False, dev="
     lengths = [s + n for s, n in zip(starts, news)]
     pools, table, kf, vf = build_pools(seqs, lengths, H, D, fill, g, fp8=fp8, dev=dev,
                                        stored=starts if fp8 else lengths)
-    if fp8 and bf16_tiles:       # dequant_fp8x16: the fp32 product, rounded to bf16
+    if fp8 and bf16_tiles:       # kv_dequantize_kernel: the fp32 product, rounded to bf16
         kf, vf = ((c.float().cpu() * s.cpu().unsqueeze(-1)).to(torch.bfloat16).double() for c, s in
                   ((pools[0], pools[2]), (pools[1], pools[3])))
     qkv = torch.cat([torch.stack([q, k[:, s:], v[:, s:]], 2).transpose(0, 1).reshape(n, H * 3 * D)
@@ -858,13 +858,14 @@ NEWS = [1, 2, 127, 128, 129, 1000]
 
 
 @gpu
-@pytest.mark.parametrize("fp8", [False, True])
+@pytest.mark.parametrize("fp8", [False, pytest.param(True, id="fp8_staged")])
 @pytest.mark.parametrize("fill", ["nan", "decoy"])
 @pytest.mark.parametrize("regime", REGIMES)
 @pytest.mark.parametrize("D", [64, 80, 128])
 def test_paged_prefill_attention(D, regime, fill, fp8):
-    """The paged prefill kernel over bf16 pools (every position in the pools) and its FP8 form (cached positions in
-    FP8 pools, new ones from qkv), every start with every number of new tokens."""
+    """The paged prefill kernel over bf16 pools (every position in the pools) and over FP8 pools through a staging pool
+    (cached positions dequantized from the FP8 pools, new ones from qkv), every start with every number of new
+    tokens."""
     H = 4
     scale = 1 / math.sqrt(D)
     slopes = regime_slopes(regime, H)
@@ -872,7 +873,15 @@ def test_paged_prefill_attention(D, regime, fill, fp8):
     rows = [(s, n) for s in (FP8_STARTS if fp8 else STARTS) for n in NEWS]
     starts, news = [r[0] for r in rows], [r[1] for r in rows]
     qkv, pools, table, cu, st, refs = _prefill_layout(regime, H, D, starts, news, fill, g, scale, fp8=fp8, dev="cuda")
-    kw = dict(k_scales=pools[2], v_scales=pools[3]) if fp8 else {}
+    kw = {}
+    if fp8:
+        lengths = [s + n for s, n in zip(starts, news)]
+        pages = [table[r, :-(-n // PAGE_SIZE)].tolist() for r, n in enumerate(lengths)]
+        num, src, dst, slot, st_table = fp8_prefill_staging(pages, starts, lengths)
+        k_stage = torch.full((num, H, PAGE_SIZE, D), math.nan, dtype=torch.bfloat16, device="cuda")
+        dev = lambda x: torch.tensor(x, dtype=torch.int32, device="cuda")   # noqa: E731
+        kw = dict(k_scales=pools[2], v_scales=pools[3],
+                  stage=(k_stage, k_stage.clone(), dev(src), dev(dst), dev(slot), dev(st_table)))
     out = alibi_paged_prefill_attention(qkv.to(torch.bfloat16).cuda(), pools[0], pools[1], table, cu.cuda(),
                                         st.cuda(), max(news), slopes.cuda(), D, **kw).view(-1, H, D)
     fam = flash_family(D)

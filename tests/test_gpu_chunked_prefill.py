@@ -1,93 +1,13 @@
-"""Chunked prefill on the GPU: the FP8 form of the paged prefill kernel bit for bit against the staged path (the bf16
-kernel over dequantized pages) and against the fp32 reference, and ``ContinuousBatcher(chunked_prefill=True)`` against
-the training forward (teacher-forced), with bf16 and FP8 pools."""
+"""Chunked prefill on the GPU: ``ContinuousBatcher(chunked_prefill=True)`` against the training forward
+(teacher-forced), with bf16 and FP8 pools."""
 import pytest
 import torch
 
-from pipegoose_b200.ops import attention as A
-from pipegoose_b200.ops import kernels as K
-from pipegoose_b200.ops.attention import (PAGE_SIZE, alibi_paged_prefill_attention,
-                                          alibi_paged_prefill_attention_reference, fp8_prefill_staging, quantize_kv)
+from pipegoose_b200.ops.attention import PAGE_SIZE
 
 pytestmark = pytest.mark.gpu
 
 FP8 = torch.float8_e4m3fn
-
-
-def _rel(a, b):
-    a, b = a.float().cpu(), b.float().cpu()
-    return (a - b).abs().max().item() / (b.abs().max().item() + 1e-6)
-
-
-def _fp8_case(H, D, starts, news, seed, spare_pages=5):
-    """Pools of NaN codes and NaN scales with quantized random keys / values in every sequence's cached positions
-    ``0 .. starts[r] - 1``, shuffled page tables, and ``qkv`` of the new tokens; all on the CPU."""
-    g = torch.Generator().manual_seed(seed)
-    lengths = [s + n for s, n in zip(starts, news)]
-    need = [(n - 1) // PAGE_SIZE + 1 for n in lengths]
-    num_pages = sum(need) + spare_pages
-    perm = torch.randperm(num_pages, generator=g).to(torch.int32)
-    table = torch.full((len(lengths), max(need) + 1), -7, dtype=torch.int32)   # never read
-    k_pool = torch.full((num_pages, H, PAGE_SIZE, D), 0x7F, dtype=torch.uint8).view(FP8)
-    scales = torch.full((num_pages, H, PAGE_SIZE), float("nan"))
-    v_pool, k_scales, v_scales = k_pool.clone(), scales, scales.clone()
-    used = 0
-    for r, s in enumerate(starts):
-        table[r, :need[r]] = perm[used:used + need[r]]
-        used += need[r]
-        p = torch.arange(s)
-        pages, slots = table[r, p // PAGE_SIZE].long(), p % PAGE_SIZE
-        for pool, sc in ((k_pool, k_scales), (v_pool, v_scales)):
-            codes, x = quantize_kv(torch.randn(s, H, D, generator=g).to(torch.bfloat16))
-            pool[pages, :, slots], sc[pages, :, slots] = codes, x
-    qkv = torch.randn(sum(news), H * 3 * D, generator=g).to(torch.bfloat16)
-    cu = torch.tensor([0] + torch.tensor(news).cumsum(0).tolist(), dtype=torch.int32)
-    return k_pool, v_pool, k_scales, v_scales, table, qkv, cu, lengths
-
-
-@pytest.mark.parametrize("D", [64, 80, 128])
-@pytest.mark.parametrize("starts,news", [([0, 64, 192, 8192], [129, 1, 1000, 300]),
-                                         ([8192, 0, 640, 64, 128], [64, 127, 128, 513, 1])])
-def test_fp8_prefill_kernel_is_bitwise_the_staged_path(D, starts, news):
-    """Several sequences on shuffled pages, cached prefixes of 0, 1, an odd number of pages and 8192 positions, pool
-    slots past each sequence's cached positions holding NaN codes and NaN scales.  The FP8 kernel's output equals the
-    bf16 kernel's over the staging pool bit for bit, and the fp32 reference within the prefill tests' tolerance."""
-    H = 3
-    k_pool, v_pool, k_scales, v_scales, table, qkv, cu, lengths = _fp8_case(H, D, starts, news, seed=D + len(starts))
-    slopes = K.alibi_slopes(H, device="cuda")
-    gpu = [t.cuda() for t in (k_pool, v_pool, k_scales, v_scales)]
-    start = torch.tensor(starts, dtype=torch.int32)
-    args = (qkv.cuda(), gpu[0], gpu[1], table.cuda(), cu.cuda(), start.cuda(), max(news), slopes, D)
-    got = alibi_paged_prefill_attention(*args, k_scales=gpu[2], v_scales=gpu[3])
-    pages = [table[r, :(n - 1) // PAGE_SIZE + 1].tolist() for r, n in enumerate(lengths)]
-    n, src, dst, slot, st_table = fp8_prefill_staging(pages, starts, lengths)
-    k_stage = torch.full((n, H, PAGE_SIZE, D), float("nan"), dtype=torch.bfloat16, device="cuda")
-    dev = lambda x: torch.tensor(x, dtype=torch.int32, device="cuda")   # noqa: E731
-    stage = (k_stage, k_stage.clone(), dev(src), dev(dst), dev(slot), dev(st_table))
-    staged = alibi_paged_prefill_attention(*args, k_scales=gpu[2], v_scales=gpu[3], stage=stage)
-    assert torch.isfinite(got).all()
-    assert torch.equal(got.view(torch.int16), staged.view(torch.int16))
-    want = alibi_paged_prefill_attention_reference(qkv.float(), k_pool, v_pool, table, cu, start, max(news),
-                                                   slopes.cpu(), D, k_scales=k_scales, v_scales=v_scales)
-    for r in range(len(starts)):
-        assert _rel(got[cu[r]:cu[r + 1]], want[cu[r]:cu[r + 1]]) < 1e-2, (starts[r], news[r])
-    for before, after in zip((k_pool, v_pool), gpu):                      # the op does not write the pools
-        assert torch.equal(before.view(torch.uint8), after.cpu().view(torch.uint8))
-
-
-def test_fp8_prefill_kernel_refusals():
-    H, D = 2, 64
-    k_pool, v_pool, k_scales, v_scales, table, qkv, cu, _ = _fp8_case(H, D, [64], [10], seed=1)
-    slopes = K.alibi_slopes(H, device="cuda")
-    gpu = [t.cuda() for t in (k_pool, v_pool, k_scales, v_scales, qkv)]
-    with pytest.raises(ValueError, match="multiple of 64"):
-        alibi_paged_prefill_attention(gpu[4], gpu[0], gpu[1], table.cuda(), cu, torch.tensor([32], dtype=torch.int32),
-                                      10, slopes, D, k_scales=gpu[2], v_scales=gpu[3])
-    with pytest.raises(RuntimeError, match="bf16"):
-        A.native().paged_prefill_attention_fp8(gpu[4].float(), gpu[0], gpu[1], gpu[2], gpu[3], table.cuda(),
-                                               cu.cuda(), torch.tensor([64], dtype=torch.int32, device="cuda"), 10,
-                                               slopes, torch.empty(10, H * D, device="cuda", dtype=torch.bfloat16),
-                                               0.0)
 
 
 # ------------------------------------------------------------------------------------------------------------ engine
@@ -229,39 +149,3 @@ def test_chunked_fp8_engine_against_bf16_pools(arch, hidden, n_head, prefix_cach
     print(f"\nchunked fp8 vs bf16 pools, {arch} D={hidden // n_head} prefix_caching={prefix_caching}: max "
           f"teacher-forced logit distance {max(dist):.4f} of max |logit| over {len(dist)} steps")
     assert max(dist) < FP8_VS_BF16
-
-
-@pytest.mark.parametrize("chunked", [False, True])
-def test_fp8_kernel_is_bitwise_the_staged_path_on_engine_inputs(monkeypatch, chunked):
-    """Every cached-prefix prefill call of the FP8 engine (prefix hits; with chunking, every chunk) gives the same bits
-    through the FP8 kernel as through the staged path."""
-    from pipegoose_b200.serving import ContinuousBatcher
-
-    model = _model("bloom", 320, 4)
-    prompts, news = _workload(seed=17)
-    op, calls = A.alibi_paged_prefill_attention, [0]
-
-    def both(qkv, k_pool, v_pool, table, cu_seqlens, start, max_len, slopes, D, softmax_scale=0.0, k_scales=None,
-             v_scales=None, stage=None, out=None):
-        got = op(qkv, k_pool, v_pool, table, cu_seqlens, start, max_len, slopes, D, k_scales=k_scales,
-                 v_scales=v_scales)
-        if k_scales is not None:
-            cu, st, tb = cu_seqlens.tolist(), start.tolist(), table.tolist()
-            lengths = [s + cu[r + 1] - cu[r] for r, s in enumerate(st)]
-            pages = [tb[r][:(n - 1) // PAGE_SIZE + 1] for r, n in enumerate(lengths)]
-            n, src, dst, slot, st_table = fp8_prefill_staging(pages, st, lengths)
-            k_stage = torch.empty(n, k_pool.shape[1], PAGE_SIZE, D, dtype=torch.bfloat16, device="cuda")
-            dev = lambda x: torch.tensor(x, dtype=torch.int32, device="cuda")   # noqa: E731
-            stage = (k_stage, torch.empty_like(k_stage), dev(src), dev(dst), dev(slot), dev(st_table))
-            staged = op(qkv, k_pool, v_pool, table, cu_seqlens, start, max_len, slopes, D, k_scales=k_scales,
-                        v_scales=v_scales, stage=stage)
-            assert torch.equal(got.view(torch.int16), staged.view(torch.int16))
-            calls[0] += 1
-        return got if out is None else out.copy_(got)
-    monkeypatch.setattr(A, "alibi_paged_prefill_attention", both)
-    engine = ContinuousBatcher(model, max_cache_tokens=24 * PAGE_SIZE, max_prefill_tokens=128 if chunked else 400,
-                               prefix_caching=True, kv_cache_dtype=FP8, chunked_prefill=chunked)
-    for p, n in zip(prompts, news):
-        engine.submit(p, n)
-    engine.run()
-    assert engine.cached_prompt_tokens > 0 and calls[0] > 0

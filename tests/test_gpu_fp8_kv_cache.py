@@ -132,10 +132,17 @@ def test_fp8_decode_kernel_equals_bf16_kernel_on_exact_values(D):
     assert ((got - want).abs() <= 2.0 ** -7 * want.abs() + 1e-4).all(), (got - want).abs().max().item()
 
 
-@pytest.mark.parametrize("D", [64, 80, 128])
-def test_fp8_cached_prefill_matches_reference(D):
+# (starts, news) of the cached prefill: prefixes of 0, 1, 16, 65 and 2 pages; then two cases with 8192-position
+# prefixes next to short ones and new tokens crossing block boundaries
+PREFILL_CASES = [([0, 64, 1024, 4160, 128], [129, 1, 1000, 127, 128]),
+                 ([0, 64, 192, 8192], [129, 1, 1000, 300]),
+                 ([8192, 0, 640, 64, 128], [64, 127, 128, 513, 1])]
+
+
+@pytest.mark.parametrize("D,starts,news", [pytest.param(D, s, n, id=f"{D}-long{i}" if i else f"{D}")
+                                           for i, (s, n) in enumerate(PREFILL_CASES) for D in (64, 80, 128)])
+def test_fp8_cached_prefill_matches_reference(D, starts, news):
     H = 2
-    starts, news = [0, 64, 1024, 4160, 128], [129, 1, 1000, 127, 128]
     lengths = [s + n for s, n in zip(starts, news)]
     k_pool, v_pool, k_scales, v_scales, table = _fp8_case(H, D, lengths, seed=D + 4, filled=starts)
     g = torch.Generator().manual_seed(D + 5)
@@ -179,6 +186,10 @@ def test_fp8_refusals():
         alibi_paged_decode_attention(qkv, k_pool, v_pool, table, pos, 69, slopes, D)
     with pytest.raises(ValueError, match="need k_scales"):
         paged_kv_write(qkv, slot, k_pool, v_pool, D)
+    cu, start = torch.tensor([0, 1], dtype=torch.int32), torch.tensor([64], dtype=torch.int32)
+    with pytest.raises(ValueError, match="pass stage"):              # FP8 pools are read through a staging pool
+        alibi_paged_prefill_attention(qkv, k_pool, v_pool, table, cu, start, 1, slopes, D, k_scales=k_scales,
+                                      v_scales=v_scales)
     bad = {"shape": k_scales[:, :, :32].contiguous(), "dtype": k_scales.half(), "device": k_scales.cpu()}
     for what, s in bad.items():
         with pytest.raises(RuntimeError):

@@ -1,17 +1,8 @@
-"""Times chunked prefill: the FP8-reading paged prefill kernel against the staged path and the bf16 kernel, and the
-serving engine's inter-token gaps with and without chunking while long prompts arrive.
+"""Times the serving engine's inter-token gaps with and without chunked prefill while long prompts arrive.
 
-    python tools/chunked_bench.py --out profiles/chunked_prefill_h100.json [--iters 50] [--rounds 3]
+    python tools/chunked_bench.py --out profiles/chunked_prefill_h100.json [--rounds 3] [--chunk 1024]
 
-Kernel: the cached-prefill grid of tools/fp8_kv_bench.py (8 sequences of H = 16 heads, D in {64, 128}, a cached prefix
-of {1024, 8192} positions and {64, 512} new tokens on shuffled pages), plus a cached prefix of 0, where the FP8 kernel
-copies only new tokens from ``qkv`` and no page is dequantized.  Three arms, each the pool write of the new
-tokens then the attention, timed with CUDA events over ``--iters`` calls and alternated for ``--rounds`` rounds (the
-median is kept): the FP8 kernel over FP8 pools, the staged path over the same FP8 pools (cached pages dequantized into
-a bf16 staging pool, the bf16 kernel on it; the plan is uploaded outside the timed region), and the bf16 kernel over
-bf16 pools.  The FP8 kernel's output is compared with the staged path's bit for bit.
-
-Engine: random-init bf16 bloom-560m (D = 64) and bloom-3b (D = 80), pools of bf16 or FP8, chunking off (the default
+Random-init bf16 bloom-560m (D = 64) and bloom-3b (D = 80), pools of bf16 or FP8, chunking off (the default
 ``max_prefill_tokens`` = 8192: a longer prompt runs alone) or on (``max_prefill_tokens`` = ``--chunk``).  A steady
 decode load of 64 greedy requests (prompts of 32 tokens, 256 new tokens each) runs while four long prompts of 4096,
 8192, 12288 and 16384 tokens (16 new tokens each) arrive, one every 24 steps from step 24.  Reported: p50 / p99 /
@@ -32,79 +23,11 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from decode_bench import card, time_us  # noqa: E402
+from decode_bench import card  # noqa: E402
 
 SHORT, SHORT_PROMPT, SHORT_NEW = 64, 32, 256
 LONG = (4096, 8192, 12288, 16384)
 LONG_NEW, LONG_EVERY = 16, 24
-
-
-def _alternate(fns, iters, rounds):
-    times = [[] for _ in fns]
-    for _ in range(rounds):
-        for t, fn in zip(times, fns):
-            t.append(time_us(fn, iters))
-    return [statistics.median(t) for t in times]
-
-
-def kernel_rows(iters: int, rounds: int):
-    import torch
-
-    from pipegoose_b200.ops import kernels as K
-    from pipegoose_b200.ops.attention import (PAGE_SIZE, alibi_paged_prefill_attention, fp8_prefill_staging,
-                                              paged_kv_write, quantize_kv)
-
-    rows = []
-    R, H = 8, 16
-    for D in (64, 128):
-        for prefix in (0, 1024, 8192):
-            for new in (64, 512):
-                total = prefix + new
-                per = -(-total // PAGE_SIZE)
-                g = torch.Generator(device="cuda").manual_seed(prefix + new + D)
-                k_pool = torch.randn(R * per, H, PAGE_SIZE, D, device="cuda", generator=g).to(torch.bfloat16)
-                v_pool = torch.randn(R * per, H, PAGE_SIZE, D, device="cuda", generator=g).to(torch.bfloat16)
-                k8, ks = quantize_kv(k_pool)
-                v8, vs = quantize_kv(v_pool)
-                perm = torch.randperm(R * per, generator=torch.Generator().manual_seed(D)).tolist()
-                pages = [perm[r * per:(r + 1) * per] for r in range(R)]
-                dev = lambda x: torch.tensor(x, dtype=torch.int32, device="cuda")   # noqa: E731
-                table = dev(pages)
-                slot = dev([pages[r][p // PAGE_SIZE] * PAGE_SIZE + p % PAGE_SIZE
-                            for r in range(R) for p in range(prefix, total)])
-                cu = dev([r * new for r in range(R + 1)])
-                start = dev([prefix] * R)
-                qkv = torch.randn(R * new, H * 3 * D, device="cuda", generator=g).to(torch.bfloat16)
-                slopes = K.alibi_slopes(H, device="cuda")
-                n, src, dst, st_slot, st_table = fp8_prefill_staging(pages, [prefix] * R, [total] * R)
-                k_st = torch.empty(n, H, PAGE_SIZE, D, device="cuda", dtype=torch.bfloat16)
-                stage = (k_st, torch.empty_like(k_st), dev(src), dev(dst), dev(st_slot), dev(st_table))
-
-                def fp8():
-                    paged_kv_write(qkv, slot, k8, v8, D, k_scales=ks, v_scales=vs)
-                    return alibi_paged_prefill_attention(qkv, k8, v8, table, cu, start, new, slopes, D, k_scales=ks,
-                                                         v_scales=vs)
-
-                def staged():
-                    paged_kv_write(qkv, slot, k8, v8, D, k_scales=ks, v_scales=vs)
-                    return alibi_paged_prefill_attention(qkv, k8, v8, table, cu, start, new, slopes, D, k_scales=ks,
-                                                         v_scales=vs, stage=stage)
-
-                def bf16():
-                    paged_kv_write(qkv, slot, k_pool, v_pool, D)
-                    return alibi_paged_prefill_attention(qkv, k_pool, v_pool, table, cu, start, new, slopes, D)
-
-                got, ref = fp8(), staged()
-                t8, tst, t16 = _alternate([fp8, staged, bf16], iters, rounds)
-                row = {"R": R, "H": H, "D": D, "prefix": prefix, "new": new, "fp8_kernel_us": round(t8, 2),
-                       "fp8_staged_us": round(tst, 2), "bf16_us": round(t16, 2),
-                       "staged_over_fp8_kernel": round(tst / t8, 3), "fp8_kernel_over_bf16": round(t8 / t16, 3),
-                       "bitwise_equal_to_staged": bool(torch.equal(got.view(torch.int16), ref.view(torch.int16)))}
-                print(json.dumps(row), flush=True)
-                rows.append(row)
-                del k_pool, v_pool, k8, v8, ks, vs, stage, k_st
-                torch.cuda.empty_cache()
-    return rows
 
 
 def run_engine(model, dtype, chunk):
@@ -191,20 +114,15 @@ def engine_rows(chunk: int, rounds: int):
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--out", default="chunked_bench.json")
-    ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--chunk", type=int, default=1024, help="max_prefill_tokens of the chunked engine")
-    ap.add_argument("--skip-engine", action="store_true")
     args = ap.parse_args()
     sys.path.insert(0, ROOT)
     import torch
 
     if not torch.cuda.is_available():
         raise SystemExit("chunked_bench.py measures on a GPU; none is visible")
-    result = {"card": card(), "kernel": kernel_rows(args.iters, args.rounds)}
-    if not args.skip_engine:
-        result["engine"] = engine_rows(args.chunk, args.rounds)
-    result["card_after"] = card()
+    result = {"card": card(), "engine": engine_rows(args.chunk, args.rounds), "card_after": card()}
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
     with open(args.out, "w") as f:
         json.dump(result, f, indent=1)
