@@ -737,6 +737,80 @@ void paged_kv_dequantize(const torch::Tensor& k_pool, const torch::Tensor& v_poo
                                      (int)k_pool.size(3), cur_stream()) == 0, "paged_kv_dequantize failed");
 }
 
+// Beam-search forks: slots 0 .. count - 1 of page src into page dst, for every pair (int32 [n, 3]: src, dst, count)
+// and every layer of the pools [n_layer, pages, H, 64, D] (bf16, or FP8 codes with fp32 scales [n_layer, pages, H,
+// 64]).  The caller guarantees that every id is a page of the pools and that no dst is also a src.
+void paged_kv_copy(const torch::Tensor& pairs, torch::Tensor k_pools, torch::Tensor v_pools,
+                   const c10::optional<torch::Tensor>& k_scales, const c10::optional<torch::Tensor>& v_scales) {
+  PG_CUDA(pairs); PG_CUDA(k_pools); PG_CUDA(v_pools);
+  TORCH_CHECK(pairs.scalar_type() == torch::kInt32 && pairs.dim() == 2 && pairs.size(1) == 3 && pairs.is_contiguous(),
+              "paged_kv_copy: pairs must be contiguous int32 [n, 3] (src, dst, count)");
+  TORCH_CHECK(k_pools.dim() == 5 && v_pools.sizes() == k_pools.sizes() && k_pools.size(3) == 64 &&
+              k_pools.scalar_type() == v_pools.scalar_type() && k_pools.is_contiguous() && v_pools.is_contiguous(),
+              "paged_kv_copy: k_pools / v_pools must be contiguous [n_layer, pages, H, 64, D] of one dtype");
+  const bool fp8 = k_pools.scalar_type() == torch::kFloat8_e4m3fn;
+  TORCH_CHECK(fp8 || k_pools.scalar_type() == torch::kBFloat16, "paged_kv_copy: pools must be bf16 or float8_e4m3fn");
+  TORCH_CHECK(fp8 == k_scales.has_value() && fp8 == v_scales.has_value(),
+              "paged_kv_copy: float8_e4m3fn pools need k_scales and v_scales, and bf16 pools take none");
+  if (fp8) {
+    for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&*k_scales, &*v_scales}) {
+      PG_CUDA((*t)); PG_F32((*t));
+      TORCH_CHECK(t->sizes() == k_pools.sizes().slice(0, 4) && t->is_contiguous() && t->device() == k_pools.device(),
+                  "paged_kv_copy: scales must be contiguous fp32 [n_layer, pages, H, 64] like the pools");
+    }
+  }
+  const int64_t row_bytes = k_pools.size(4) * k_pools.element_size();
+  TORCH_CHECK(row_bytes % 16 == 0, "paged_kv_copy: a pool row of ", row_bytes, " bytes is not a whole number of 16-byte words");
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&pairs, &v_pools})
+    TORCH_CHECK(t->device() == k_pools.device(), "paged_kv_copy: tensors on different devices");
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&k_pools, &v_pools})
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, "paged_kv_copy: pools must be 16B aligned");
+  c10::cuda::CUDAGuard guard(k_pools.device());
+  TORCH_CHECK(pg_paged_kv_copy(pairs.data_ptr<int>(), k_pools.data_ptr(), v_pools.data_ptr(),
+                               fp8 ? k_scales->data_ptr<float>() : nullptr, fp8 ? v_scales->data_ptr<float>() : nullptr,
+                               (int)pairs.size(0), (int)k_pools.size(0), (int)k_pools.size(1), (int)k_pools.size(2),
+                               (int)row_bytes, cur_stream()) == 0, "paged_kv_copy failed");
+}
+
+// Beam search's candidate choice (csrc/beam_sm90.cu): per request r (rows cu[r] .. cu[r+1] - 1 of logits [N, V], bf16
+// or fp32, unit inner stride) the k best (score, token, row), written to out_score / out_token / out_row [R, k], and
+// each row's logsumexp into lse [N] when given.  max_rows is the host's bound on one request's rows.
+void beam_topk(const torch::Tensor& logits, const torch::Tensor& scores, const torch::Tensor& cu, int64_t k,
+               int64_t max_rows, torch::Tensor out_score, torch::Tensor out_token, torch::Tensor out_row,
+               const c10::optional<torch::Tensor>& lse, torch::Tensor ticket) {
+  TORCH_CHECK(logits.is_cuda(), "beam_topk: logits must be a CUDA tensor");
+  PG_CUDA(scores); PG_F32(scores); PG_CUDA(cu); PG_CUDA(out_score); PG_F32(out_score);
+  PG_CUDA(out_token); PG_CUDA(out_row); PG_CUDA(ticket);
+  const bool fp32 = logits.scalar_type() == torch::kFloat32;
+  TORCH_CHECK(fp32 || logits.scalar_type() == torch::kBFloat16, "beam_topk: logits must be bf16 or fp32");
+  TORCH_CHECK(logits.dim() == 2 && logits.stride(1) == 1 && logits.size(0) >= 1,
+              "beam_topk: logits must be [N, V] with unit inner stride");
+  const int64_t N = logits.size(0), V = logits.size(1), R = cu.numel() - 1;
+  TORCH_CHECK(cu.scalar_type() == torch::kInt32 && R >= 1 && cu.is_contiguous(), "beam_topk: cu must be int32 [R + 1]");
+  TORCH_CHECK(out_token.scalar_type() == torch::kInt32 && out_row.scalar_type() == torch::kInt32 &&
+              ticket.scalar_type() == torch::kInt32, "beam_topk: out_token, out_row and ticket must be int32");
+  TORCH_CHECK(scores.numel() == N && scores.is_contiguous(), "beam_topk: scores must be fp32 [N]");
+  TORCH_CHECK(1 <= k && k <= 16 && k <= V, "beam_topk: k must be in 1 .. min(16, V), got ", k);
+  TORCH_CHECK(1 <= max_rows && max_rows <= 64, "beam_topk: a request holds 1 .. 64 rows, got ", max_rows);
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&out_score, &out_token, &out_row})
+    TORCH_CHECK(t->numel() == R * k && t->is_contiguous(), "beam_topk: outputs must be contiguous [R, k]");
+  TORCH_CHECK(ticket.numel() >= R, "beam_topk: ticket must hold at least R = ", R, " entries");
+  if (lse.has_value()) {
+    PG_CUDA((*lse)); PG_F32((*lse));
+    TORCH_CHECK(lse->numel() == N && lse->is_contiguous(), "beam_topk: lse must be fp32 [N]");
+  }
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&scores, &cu, &out_score, &out_token, &out_row, &ticket})
+    TORCH_CHECK(t->device() == logits.device(), "beam_topk: tensors on different devices");
+  c10::cuda::CUDAGuard guard(logits.device());
+  const int splits = pg_beam_topk_splits((int)N, (int)V, (int)k, (int)max_rows);
+  torch::Tensor part = torch::empty({N * splits * (2 + 2 * pg_beam_topk_kp((int)k))}, scores.options());
+  TORCH_CHECK(pg_beam_topk(logits.data_ptr(), fp32 ? 1 : 0, logits.stride(0), scores.data_ptr<float>(), cu.data_ptr<int>(),
+                           part.data_ptr<float>(), ticket.data_ptr<int>(), out_score.data_ptr<float>(),
+                           out_token.data_ptr<int>(), out_row.data_ptr<int>(),
+                           lse.has_value() ? lse->data_ptr<float>() : nullptr, (int)N, (int)V, (int)R, (int)k,
+                           (int)max_rows, splits, cur_stream()) == 0, "beam_topk failed");
+}
+
 void moe_route(const torch::Tensor& x, const torch::Tensor& wg, const c10::optional<torch::Tensor>& bg,
                const c10::optional<torch::Tensor>& jitter, int64_t top_k, int64_t capacity, torch::Tensor probs,
                torch::Tensor topk_idx, torch::Tensor topk_prob, torch::Tensor pos, torch::Tensor counts,
@@ -938,6 +1012,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("max_pos"), py::arg("slopes"), py::arg("out"), py::arg("ticket"), py::arg("softmax_scale") = 0.0);
   m.def("paged_kv_dequantize", &paged_kv_dequantize, py::arg("k_pool"), py::arg("v_pool"), py::arg("k_scales"),
         py::arg("v_scales"), py::arg("src"), py::arg("dst"), py::arg("k_out"), py::arg("v_out"));
+  m.def("paged_kv_copy", &paged_kv_copy, py::arg("pairs"), py::arg("k_pools"), py::arg("v_pools"),
+        py::arg("k_scales") = py::none(), py::arg("v_scales") = py::none());
+  m.def("beam_topk", &beam_topk, py::arg("logits"), py::arg("scores"), py::arg("cu"), py::arg("k"), py::arg("max_rows"),
+        py::arg("out_score"), py::arg("out_token"), py::arg("out_row"), py::arg("lse"), py::arg("ticket"));
   m.def("moe_route", &moe_route);
   m.def("moe_dispatch", &moe_dispatch);
   m.def("symm_alloc", &symm_alloc);

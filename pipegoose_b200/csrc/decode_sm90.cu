@@ -24,11 +24,16 @@
 // every row has its own position pos[b] (int32 [B] on the device).  Row b's position p lives in page
 // table[b, p / 64] (int32 [B, max_pages]) at slot p % 64.  Row b writes its new k / v into the slot of pos[b] and
 // attends to keys 0 <= k <= pos[b]; there is no lead.  The grid is sized for the longest row (`pos` holds the host's
-// bound on max(pos[b])); each row cuts its own range into `splits` chunks, so the bound only shapes the grid.  Rows
-// own disjoint pages, so the write of pos[b]'s slot races no read either.
+// bound on max(pos[b])); each row cuts its own range into `splits` chunks, so the bound only shapes the grid.  The page
+// holding pos[b] belongs to row b alone; other pages may be shared between rows and are only read.  So the write of
+// pos[b]'s slot races no read either.
 //
 // paged_kv_write_kernel stores the k / v of a packed prefill into the pools: token n's heads go to slot[n]
 // (page * 64 + offset), 16 bytes per thread.
+//
+// paged_kv_copy_kernel copies the leading slots of pages (beam search forks a shared partly filled page): for every
+// pair i = (src, dst, count) and every layer of the [n_layer, pages, H, 64, D] pools, slots 0 .. count - 1 of K and V
+// of page src go to page dst, 16 bytes per thread, with their fp32 scales over FP8 pools.
 //
 // FP8 pools (e4m3 codes [num_pages, H, 64, D] and fp32 scales [num_pages, H, 64], one per position, head and K | V):
 // a row x of D values is stored as scale = amax / 448 and code_i = e4m3_rn_satfinite(x_i * (448 / amax)), all codes 0
@@ -457,6 +462,36 @@ __global__ void __launch_bounds__(256) paged_kv_write_kernel(const uint4* __rest
   (kv ? v_pool : k_pool)[dst] = x;
 }
 
+// One thread per (pair, layer, head, K|V, slot, 16-byte column); threads of slots >= count return at once.  The column-0
+// thread of a row also copies its scale (FP8 pools).
+__global__ void __launch_bounds__(256) paged_kv_copy_kernel(const int* __restrict__ pairs, uint4* __restrict__ k_pools,
+                                                            uint4* __restrict__ v_pools, float* __restrict__ k_scales,
+                                                            float* __restrict__ v_scales, int n, int layers,
+                                                            int pages, int H, int vec) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<long long>(n) * layers * H * 2 * kPageSize * vec) return;
+  const int c = static_cast<int>(i % vec);
+  long long r = i / vec;
+  const int slot = static_cast<int>(r % kPageSize);
+  r /= kPageSize;
+  const int kv = static_cast<int>(r & 1);
+  r >>= 1;
+  const int h = static_cast<int>(r % H);
+  r /= H;
+  const int layer = static_cast<int>(r % layers);
+  const int p = static_cast<int>(r / layers);
+  if (slot >= __ldg(pairs + 3 * p + 2)) return;
+  const long long base = static_cast<long long>(layer) * pages;
+  const size_t from = ((base + __ldg(pairs + 3 * p)) * H + h) * kPageSize + slot;
+  const size_t to = ((base + __ldg(pairs + 3 * p + 1)) * H + h) * kPageSize + slot;
+  uint4* pool = kv ? v_pools : k_pools;
+  pool[to * vec + c] = pool[from * vec + c];
+  float* scales = kv ? v_scales : k_scales;
+  if (c == 0 && scales != nullptr) scales[to] = scales[from];
+}
+
 // ---- FP8 pools
 constexpr float kFp8Max = 448.0f;   // largest finite e4m3
 
@@ -859,5 +894,19 @@ extern "C" int pg_paged_kv_dequantize(const void* k_pool, const void* v_pool, co
                  static_cast<uint4*>(k_out), static_cast<uint4*>(v_out), n, H * kPageSize, D / 16) != cudaSuccess)
     return -1;
   PG_CHECK_LAUNCH("kv_dequantize");
+  return 0;
+}
+
+extern "C" int pg_paged_kv_copy(const int* pairs, void* k_pools, void* v_pools, float* k_scales, float* v_scales, int n,
+                                int layers, int pages, int H, int row_bytes, cudaStream_t s) {
+  if (n < 0 || layers < 1 || pages < 1 || H < 1 || row_bytes % 16 != 0 || (k_scales == nullptr) != (v_scales == nullptr))
+    return -1;
+  if (n == 0) return 0;
+  const long long threads = static_cast<long long>(n) * layers * H * 2 * kPageSize * (row_bytes / 16);
+  if (launch_pdl(paged_kv_copy_kernel, dim3(static_cast<unsigned>((threads + 255) / 256)), dim3(256), 0, s, pairs,
+                 static_cast<uint4*>(k_pools), static_cast<uint4*>(v_pools), k_scales, v_scales, n, layers, pages, H,
+                 row_bytes / 16) != cudaSuccess)
+    return -1;
+  PG_CHECK_LAUNCH("paged_kv_copy");
   return 0;
 }

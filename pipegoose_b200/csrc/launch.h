@@ -145,6 +145,23 @@ int pg_paged_decode_attention_fp8(const void* qkv, void* k_pool, void* v_pool, f
 int pg_paged_kv_dequantize(const void* k_pool, const void* v_pool, const float* k_scales, const float* v_scales,
                            const int* src, const int* dst, void* k_out, void* v_out, int n, int H, int D,
                            cudaStream_t s);
+// Beam-search forks: for every pair i of pairs (int32 [n, 3]: src page, dst page, count) and every layer of the pools
+// k_pools / v_pools [layers, pages, H, 64, D] (row_bytes = D * element size), slots 0 .. count - 1 of page src are
+// copied into page dst, with their fp32 scales [layers, pages, H, 64] when k_scales / v_scales are given (FP8 pools).
+int pg_paged_kv_copy(const int* pairs, void* k_pools, void* v_pools, float* k_scales, float* v_scales, int n,
+                     int layers, int pages, int H, int row_bytes, cudaStream_t s);
+
+// ---- beam_sm90.cu
+// Beam search's candidate choice: for every request r (rows cu[r] .. cu[r+1] - 1 of logits [N, V], bf16 or, with
+// fp32 != 0, fp32, row stride ld) the k (1 .. 16) best (score, token, row) by score = scores[row] + (logit - lse[row]),
+// descending, ties to the lower (row, token); lse (nullable, fp32 [N]) receives each row's logsumexp.  max_rows
+// (<= 64) bounds the rows of one request; splits comes from pg_beam_topk_splits(N, V, k, max_rows).  part holds
+// N * splits * (2 + 2 * pg_beam_topk_kp(k)) floats; ticket is an int32 [R] array, zero before the call and after it.
+int pg_beam_topk_kp(int k);
+int pg_beam_topk_splits(int N, int V, int k, int max_rows);
+int pg_beam_topk(const void* logits, int fp32, long long ld, const float* scores, const int* cu, float* part,
+                 int* ticket, float* out_score, int* out_token, int* out_row, float* lse, int N, int V, int R, int k,
+                 int max_rows, int splits, cudaStream_t s);
 
 // ---- moe.cu
 int pg_moe_route(const void* x, const void* wg, const void* bg, const float* jitter, int n, int h, int E, int top_k,

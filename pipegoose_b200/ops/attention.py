@@ -259,7 +259,8 @@ def alibi_decode_attention(qkv_new: torch.Tensor, k_cache: torch.Tensor, v_cache
 # new-token position ``pos[b]`` (int32 ``[B]``): the step writes its k / v into that slot, and row b's query attends to
 # keys ``0 <= k <= pos[b]`` with ``q.k * scale + slope[head] * (k - pos[b])``.  ``max_pos`` is a host integer
 # ``>= max(pos)``: it sizes the kernel's grid only.  Neither op reads ``table`` or ``pos`` on the host; their caller
-# guarantees ``pos[b] <= max_pos``, that the pages a row uses are pages of the pool, and that no two rows share one.
+# guarantees ``pos[b] <= max_pos`` and that the pages a row uses are pages of the pool.  The page holding ``pos[b]``
+# belongs to row b alone; other pages may be shared between rows and are only read (prefix caching, beam search).
 #
 # FP8 pools (``ContinuousBatcher(kv_cache_dtype=torch.float8_e4m3fn)``): the pools hold ``torch.float8_e4m3fn`` codes
 # and every op takes fp32 ``k_scales`` / ``v_scales`` ``[num_pages, n_head, PAGE_SIZE]``, one scale per position and
@@ -429,6 +430,32 @@ def paged_kv_dequantize(k_pool: torch.Tensor, v_pool: torch.Tensor, k_scales: to
         return paged_kv_dequantize_reference(k_pool, v_pool, k_scales, v_scales, src, dst, k_out, v_out)
     native().paged_kv_dequantize(k_pool, v_pool, k_scales, v_scales, src.to(torch.int32).contiguous(),
                                  dst.to(torch.int32).contiguous(), k_out, v_out)
+
+
+def _copy_pairs(pairs) -> torch.Tensor:
+    return (pairs if torch.is_tensor(pairs) else torch.tensor(pairs, dtype=torch.int32)).to(torch.int32).view(-1, 3)
+
+
+def paged_kv_copy_reference(pairs, k_pools: torch.Tensor, v_pools: torch.Tensor, k_scales=None,
+                            v_scales=None) -> None:
+    """PyTorch form of :func:`paged_kv_copy`."""
+    _fp8_pools(k_pools, k_scales, v_scales)
+    for src, dst, n in _copy_pairs(pairs).tolist():
+        for t in (k_pools, v_pools) + ((k_scales, v_scales) if k_scales is not None else ()):
+            t[:, dst, :, :n] = t[:, src, :, :n]
+
+
+def paged_kv_copy(pairs, k_pools: torch.Tensor, v_pools: torch.Tensor, k_scales=None, v_scales=None) -> None:
+    """Beam-search forks: for every ``(src page, dst page, count)`` of ``pairs`` (int32 ``[n, 3]`` or a host list of
+    triples) and every layer of the pools ``[n_layer, pages, n_head, PAGE_SIZE, D]``, slots ``0 .. count-1`` of page
+    ``src`` into page ``dst``, with their scales ``[n_layer, pages, n_head, PAGE_SIZE]`` over FP8 pools; nothing else
+    changes.  No ``dst`` may also be a ``src``.  CUDA bf16 and FP8 pools run ``paged_kv_copy_kernel``, one launch for
+    all pairs and layers."""
+    fp8 = _fp8_pools(k_pools, k_scales, v_scales)
+    if not (k_pools.is_cuda and (fp8 or k_pools.dtype == torch.bfloat16)):
+        return paged_kv_copy_reference(pairs, k_pools, v_pools, k_scales, v_scales)
+    pairs = _copy_pairs(pairs).to(k_pools.device, non_blocking=True).contiguous()
+    native().paged_kv_copy(pairs, k_pools, v_pools, k_scales, v_scales)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

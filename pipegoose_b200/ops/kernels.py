@@ -385,3 +385,62 @@ def alibi_slopes(n_head: int, device=None) -> torch.Tensor:
         extra = torch.pow(torch.tensor(extra_base, dtype=torch.float32), torch.arange(1, 1 + 2 * n_rem, 2, dtype=torch.float32))
         slopes = torch.cat([slopes, extra])
     return slopes.to(device)
+
+
+# ----------------------------------------------------------------------------------------------
+# beam search's candidate choice (pipegoose_b200.serving): per request r, whose beams are rows cu_beams[r] ..
+# cu_beams[r+1]-1 of logits [N, V], the k best (score, token, row) by score = beam_score[row] + log_softmax(logits[row])
+# [token], in fp32, sorted descending; equal scores go to the lower (row, token).
+# ----------------------------------------------------------------------------------------------
+BEAM_TOPK_MAX_K = 16
+
+
+def _beam_topk_check(logits: torch.Tensor, cu: list, k: int) -> None:
+    V = logits.shape[1]
+    if not 1 <= k <= min(BEAM_TOPK_MAX_K, V):
+        raise ValueError(f"beam_topk: k must be in 1 .. min({BEAM_TOPK_MAX_K}, V = {V}), got {k}")
+    if len(cu) < 2 or cu[0] != 0 or cu[-1] != logits.shape[0] or any(b <= a for a, b in zip(cu, cu[1:])):
+        raise ValueError(f"beam_topk: cu_beams must rise from 0 to the {logits.shape[0]} rows, got {cu}")
+
+
+def beam_topk_reference(logits: torch.Tensor, scores: torch.Tensor, cu_beams, k: int, return_lse: bool = False):
+    """fp32 PyTorch form of :func:`beam_topk` (CPU path, test oracle): ``log_softmax``, the add and a stable
+    descending sort of each request's flat ``rows * V`` scores."""
+    cu = [int(c) for c in cu_beams]
+    _beam_topk_check(logits, cu, k)
+    x = logits.float()
+    lp = torch.log_softmax(x, -1) + scores.to(x.device).float().view(-1, 1)
+    V = x.shape[1]
+    out_s, out_t, out_r = [], [], []
+    for a, b in zip(cu, cu[1:]):
+        flat = lp[a:b].reshape(-1)
+        idx = torch.sort(flat, descending=True, stable=True).indices[:k]
+        out_s.append(flat[idx])
+        out_t.append(idx % V)
+        out_r.append(idx // V + a)
+    out = (torch.stack(out_s), torch.stack(out_t), torch.stack(out_r))
+    return out + (torch.logsumexp(x, -1) if return_lse else None,)
+
+
+def beam_topk(logits: torch.Tensor, scores: torch.Tensor, cu_beams, k: int, return_lse: bool = False):
+    """Beam search's candidate choice (section comment above) from ``logits [N, V]`` (bf16 or fp32, rows may be
+    strided) and fp32 running scores ``[N]``; ``cu_beams`` is a host sequence of R + 1 ints, at most 64 rows per
+    request, and ``k <= 16``.  Returns ``(scores [R, k] fp32, tokens [R, k], rows [R, k], lse [N] or None)``; rows
+    index all N rows.  CUDA logits run ``beam_topk_kernel`` (``csrc/beam_sm90.cu``), which reads the logits once."""
+    if not logits.is_cuda:
+        return beam_topk_reference(logits, scores, cu_beams, k, return_lse)
+    from pipegoose_b200.ops.attention import _decode_ticket
+
+    cu = [int(c) for c in cu_beams]
+    _beam_topk_check(logits, cu, k)
+    if logits.dtype not in (torch.bfloat16, torch.float32) or logits.stride(1) != 1:
+        raise ValueError(f"beam_topk: the kernel takes bf16 or fp32 logits with unit inner stride, got {logits.dtype}")
+    dev, R = logits.device, len(cu) - 1
+    cu_dev = torch.tensor(cu, dtype=torch.int32).to(dev, non_blocking=True)
+    out_s = torch.empty(R, k, dtype=torch.float32, device=dev)
+    out_t = torch.empty(R, k, dtype=torch.int32, device=dev)
+    out_r = torch.empty(R, k, dtype=torch.int32, device=dev)
+    lse = torch.empty(logits.shape[0], dtype=torch.float32, device=dev) if return_lse else None
+    native().beam_topk(logits, scores.to(dev).float().contiguous(), cu_dev, k, max(b - a for a, b in zip(cu, cu[1:])),
+                       out_s, out_t, out_r, lse, _decode_ticket(R, dev))
+    return out_s, out_t, out_r, lse

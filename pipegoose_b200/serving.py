@@ -88,6 +88,32 @@ alone are 256 x V model-dtype values) and a capture pause the first time a bucke
 path (CUDA bf16 weights, head size 64, 80 or 128) and ``BloomMLP`` MLPs (``ExpertLayer`` routing depends on the data):
 refused otherwise.  ``graph_decode_steps`` counts the decode steps served by a replay.
 
+Beam search (``submit(..., num_beams=W)``, 2 .. ``MAX_BEAMS`` = 8; ``num_beams=1`` is the plain request): 🤗's
+``GenerationMixin._beam_search`` per request, with ``length_penalty``, ``early_stopping`` (True, False or "never") and
+``num_return_sequences``.  Every step keeps the 2W best candidates over the request's W beams (its first step: 2W from
+the prompt's one row), sends those among the top W that end in ``eos_token_id`` (or reach ``max_new_tokens``) to the
+finished hypotheses with the length penalty on the generated length, continues with the W best of the others and stops
+by 🤗's rules.  The result is the best hypothesis; ``hypotheses[rid]`` holds the ``num_return_sequences`` best
+``(prompt + tokens, score)``, best first, with 🤗's ``sequences_scores`` as score, and the caller pops its entries.
+The beams are decode rows like any request's, through the paged decode kernel, in mixed steps and in graph replays
+(whose buckets count rows); the beam step runs eagerly after the forward, on the model-dtype logits, through one
+``beam_topk`` call (a fused log-softmax and top-k) for all beam requests and one device-to-host transfer.
+Reservation: a beam request reserves ``prompt // 64 + W * (pages - prompt // 64)`` pages at admission (the prompt's
+full pages once, the rest per beam) and is admitted, and releases every page, like any request, so nothing is ever
+preempted; ``submit`` refuses it if that exceeds the pool.  Forks: inside the request its reserved pages are shared out
+among its beams with request-local reference counts.  After a beam step every new beam takes its parent's page list
+(references are taken before the old beams' are dropped).  Copy-on-write: the page holding a beam's next write
+position ``len(tokens) - 1`` must be that beam's alone; the first of its holders in 🤗's order keeps it, every other
+gets a page from the request's reserve with the leading ``pos % 64`` slots copied, and at ``pos % 64 == 0`` the write
+starts a fresh page.  One ``paged_kv_copy`` launch per step copies every such page in every layer (with its scales
+over FP8 pools); ``beam_page_copies`` counts them.  A request that would need more pages than it reserved raises
+``RuntimeError``.  With prefix caching a beam request takes its prompt's hits as any request does and indexes its
+prompt's pages only, never beam pages.  Beam requests work with prefix caching, FP8 pools, chunked prefill and
+``cuda_graphs``, beside greedy and sampled requests, whose tokens do not depend on them (up to the rounding a graph
+bucket or cuBLAS's choice for another M brings, as above).  Refused: ``num_beams`` outside 1 .. 8, ``do_sample=True``
+with ``num_beams > 1`` (beam sampling), ``num_return_sequences`` outside 1 .. ``num_beams``, ``2 * num_beams`` above the
+vocabulary, and beam requests on an engine with speculative decoding.
+
 Limits: sampled tokens depend on which requests share a step (the random stream is consumed per group; in a verify
 step a group takes one uniform number per token row, then one draw per row without the draft, then one per row);
 an ``ExpertLayer`` capacity limit counts the tokens of one step, as in ``generate()`` (with prefix caching, cached keys
@@ -101,6 +127,7 @@ import itertools
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from pipegoose_b200.ops.attention import APPEND_MAX_TOKENS, PAGE_SIZE, fp8_prefill_staging
@@ -108,6 +135,7 @@ from pipegoose_b200.ops.attention import APPEND_MAX_TOKENS, PAGE_SIZE, fp8_prefi
 SPEC_NGRAM_SIZES = (3, 2)                           # trailing n-gram sizes the drafter looks up, longest first
 MAX_SPECULATIVE_TOKENS = APPEND_MAX_TOKENS - 1      # drafts per request and step: with the last token, one append
 GRAPH_BATCH_SIZES = (1, 2, 4, 8, 16, 32, 64, 128, 256)   # decode batch buckets captured as CUDA graphs (cuda_graphs)
+MAX_BEAMS = 8                                       # num_beams of one request: its 2 * num_beams candidates per step
 
 
 class _NgramIndex:
@@ -139,6 +167,31 @@ class _NgramIndex:
 
 
 @dataclass
+class _Beam:
+    """One running beam of a beam-search request: its tokens (prompt + generated), fp32 running score and pages."""
+    tokens: List[int]
+    score: float
+    pages: List[int]
+
+
+@dataclass
+class _BeamSearch:
+    """A beam-search request's state.  ``beams`` are its decode rows in 🤗's order (one row, the prompt, before its
+    first beam step); ``finished`` its best finished hypotheses ``(score, generated tokens)``, best first, at most
+    ``width``; ``refs`` the request-local references of the pages its beams hold and ``spare`` its reserved pages that
+    no beam holds."""
+    width: int
+    length_penalty: float
+    early_stopping: object            # True, False or "never"
+    num_return_sequences: int
+    beams: List[_Beam] = field(default_factory=list)
+    finished: List[Tuple[float, List[int]]] = field(default_factory=list)
+    improvable: bool = True           # 🤗's early-stopping heuristic: can a running beam still beat the worst finished
+    refs: Dict[int, int] = field(default_factory=dict)
+    spare: List[int] = field(default_factory=list)
+
+
+@dataclass
 class _Request:
     rid: int
     tokens: List[int]
@@ -150,10 +203,21 @@ class _Request:
     cached: int = 0            # prompt positions served from the prefix cache (a multiple of the page size)
     filled: int = 0            # chunked prefill: prompt positions in the cache so far (at least ``cached``)
     ngrams: Optional[_NgramIndex] = None      # speculative decoding only
+    beam: Optional[_BeamSearch] = None        # beam search only
 
     @property
     def pages_needed(self) -> int:
-        return -(-(self.prompt_len + self.max_new_tokens) // PAGE_SIZE)
+        """Pages reserved at admission: those of the whole sequence; for beam search the prompt's full pages once and
+        the rest once per beam."""
+        n = -(-(self.prompt_len + self.max_new_tokens) // PAGE_SIZE)
+        if self.beam is None:
+            return n
+        full = self.prompt_len // PAGE_SIZE
+        return full + self.beam.width * (n - full)
+
+    def rows(self) -> list:
+        """The request's decode rows (objects with ``tokens`` and ``pages``): its beams, or itself."""
+        return self.beam.beams if self.beam is not None else [self]
 
 
 class ContinuousBatcher:
@@ -173,7 +237,10 @@ class ContinuousBatcher:
     speculative decoding.
     ``cuda_graphs``: replay plain decode steps of at most ``GRAPH_BATCH_SIZES[-1]`` requests from CUDA graphs, one per
     batch bucket, captured on first use (module docstring); costs the graphs' memory pool and one capture pause per
-    bucket.  Needs a model on the native decode path with ``BloomMLP`` MLPs."""
+    bucket.  Needs a model on the native decode path with ``BloomMLP`` MLPs.
+
+    Beam search: ``submit(..., num_beams=W)`` (module docstring); ``hypotheses`` maps a finished beam request's id to
+    its best ``(prompt + tokens, score)``, and ``beam_page_copies`` counts the partial pages its forks copied."""
 
     def __init__(self, model, max_cache_tokens: int, max_prefill_tokens: int = 8192,
                  generator: Optional[torch.Generator] = None, prefix_caching: bool = False,
@@ -214,6 +281,10 @@ class ContinuousBatcher:
                              f"128 (got {w.dtype} on {w.device}, head size {D})")
         self.cuda_graphs = bool(cuda_graphs)
         self.graph_decode_steps = 0                               # decode steps served by a graph replay
+        self._native = _native_decode(w, D)
+        self.vocab_size = model.lm_head.weight.shape[0]
+        self.beam_page_copies = 0                                 # partial pages copied by beam forks
+        self.hypotheses: Dict[int, List[Tuple[List[int], float]]] = {}   # beam search: rid -> best hypotheses
         self.chunked_prefill = bool(chunked_prefill)
         self.num_speculative_tokens = int(num_speculative_tokens)
         self.speculative_proposed_tokens = 0                      # drafts verified
@@ -254,23 +325,44 @@ class ContinuousBatcher:
 
     # ------------------------------------------------------------------ public
     def submit(self, prompt_ids: Sequence[int], max_new_tokens: int, do_sample: bool = False, temperature: float = 1.0,
-               top_k: int = 0, top_p: float = 1.0, eos_token_id: Optional[int] = None) -> int:
-        """Queue one request; returns its id.  The arguments mean what they mean in ``generate()``."""
+               top_k: int = 0, top_p: float = 1.0, eos_token_id: Optional[int] = None, num_beams: int = 1,
+               length_penalty: float = 1.0, early_stopping=False, num_return_sequences: int = 1) -> int:
+        """Queue one request; returns its id.  The arguments mean what they mean in ``generate()`` and 🤗's beam
+        search (module docstring).  With ``num_beams > 1`` the request's result is its best hypothesis, and
+        ``hypotheses[rid]`` receives its ``num_return_sequences`` best ``(prompt + tokens, score)``, best first, where the
+        score is 🤗's ``sequences_scores``; the caller pops those entries."""
         tokens = [int(t) for t in (prompt_ids.reshape(-1).tolist() if torch.is_tensor(prompt_ids) else prompt_ids)]
         if not tokens:
             raise ValueError("empty prompt: a request needs at least one token")
         if max_new_tokens < 1:
             raise ValueError(f"max_new_tokens must be at least 1, got {max_new_tokens}")
+        if not 1 <= num_beams <= MAX_BEAMS:
+            raise ValueError(f"num_beams must be in 1 .. {MAX_BEAMS}, got {num_beams}")
+        if not 1 <= num_return_sequences <= num_beams:
+            raise ValueError(f"num_return_sequences must be in 1 .. num_beams = {num_beams}, got {num_return_sequences}")
+        beam = None
+        if num_beams > 1:
+            if do_sample:
+                raise ValueError("num_beams > 1 does not support do_sample=True (beam sampling)")
+            if self.num_speculative_tokens:
+                raise ValueError("num_beams > 1 is not supported with speculative decoding (num_speculative_tokens > 0)")
+            if early_stopping not in (True, False, "never"):
+                raise ValueError(f"early_stopping must be True, False or 'never', got {early_stopping!r}")
+            if 2 * num_beams > self.vocab_size:
+                raise ValueError(f"num_beams = {num_beams} needs 2 * num_beams candidates per step; the vocabulary has "
+                                 f"{self.vocab_size} tokens")
+            beam = _BeamSearch(int(num_beams), float(length_penalty), early_stopping, int(num_return_sequences))
         # the last new token is never fed back: positions 0 .. prompt + max_new_tokens - 2 are embedded
         if self.n_positions is not None and len(tokens) + max_new_tokens - 1 > self.n_positions:
             raise ValueError(f"prompt ({len(tokens)}) + max_new_tokens ({max_new_tokens}) - 1 positions exceed the "
                              f"model's n_positions = {self.n_positions}")
         r = _Request(next(self._ids), tokens, len(tokens), int(max_new_tokens),
                      (bool(do_sample), float(temperature), int(top_k), float(top_p)) if do_sample else (False,),
-                     eos_token_id)
+                     eos_token_id, beam=beam)
         if r.pages_needed > self.num_pages:
+            what = f" with num_beams {num_beams}" if beam is not None else ""
             raise ValueError(f"the request needs {r.pages_needed} pages of {PAGE_SIZE} positions (prompt {len(tokens)} + "
-                             f"max_new_tokens {max_new_tokens}); the pool has {self.num_pages}")
+                             f"max_new_tokens {max_new_tokens}{what}); the pool has {self.num_pages}")
         self._waiting.append(r)
         return r.rid
 
@@ -282,14 +374,19 @@ class ContinuousBatcher:
         that finished."""
         self._admit()
         spec = self._speculate() if self.num_speculative_tokens and not self._admitted else None
+        done = []
         if spec is not None:
             reqs, emitted = spec
         else:
-            reqs, logits = self._forward()
-            if not reqs:
+            rows, logits = self._forward()
+            if not rows:
                 return []
-            emitted = [[t] for t in self._select(reqs, logits)]
-        done = []
+            reqs = [r for r in rows if r.beam is None]              # plain rows come first (_order)
+            emitted = [[t] for t in self._select(reqs, logits[:len(reqs)].float())] if reqs else []
+            tail = rows[len(reqs):]                                 # beam requests, each with its rows adjacent
+            beams = [r for i, r in enumerate(tail) if i == 0 or tail[i - 1] is not r]
+            if beams:
+                done = self._beam_step(beams, logits[len(reqs):])
         for r, new in zip(reqs, emitted):
             r.tokens += new
             if len(r.tokens) - r.prompt_len == r.max_new_tokens or new[-1] == r.eos_token_id:
@@ -311,6 +408,11 @@ class ContinuousBatcher:
         return outs
 
     # ------------------------------------------------------------------ internals
+    @staticmethod
+    def _order(r: _Request) -> Tuple:
+        """Row order of a step: requests that share sampling parameters adjacent, beam-search requests last."""
+        return (r.beam is not None, r.sampling)
+
     def _admit(self) -> None:
         if self.prefix_caching:
             return self._admit_cached()
@@ -380,8 +482,8 @@ class ContinuousBatcher:
 
     def _release(self, r: _Request) -> None:
         """A finished request: index the pages its generated tokens filled (positions up to ``len(tokens) - 2`` are in
-        the cache), then drop its references, last page first."""
-        self._register(r, len(r.tokens) - 1)
+        the cache; a beam-search request indexes its prompt only), then drop its references, last page first."""
+        self._register(r, r.prompt_len if r.beam is not None else len(r.tokens) - 1)
         for p in reversed(r.pages):
             self._refs[p] -= 1
             if self._refs[p] == 0:
@@ -393,8 +495,8 @@ class ContinuousBatcher:
         return list(flat.split([len(r) for r in rows]))
 
     def _forward(self) -> Tuple[List[_Request], torch.Tensor]:
-        """The requests this step serves, with requests that share sampling parameters adjacent, and their fp32
-        next-token logits ``[len(reqs), V]``."""
+        """The owner of every row this step serves (a beam-search request owns one row per beam), in ``_order``, and
+        the rows' next-token logits ``[len(rows), V]`` in the model's dtype."""
         if self._admitted and self.chunked_prefill:
             return self._mixed()
         if self._admitted:                                      # prefill the oldest admitted prompts
@@ -403,27 +505,29 @@ class ContinuousBatcher:
                                       <= self.max_prefill_tokens):
                 reqs.append(self._admitted.popleft())
                 n += reqs[-1].prompt_len - reqs[-1].cached
-            reqs.sort(key=lambda r: r.sampling)
+            reqs.sort(key=self._order)
             if self.prefix_caching:
                 logits = self._prefill_cached(reqs) if any(r.cached for r in reqs) else self._prefill(reqs)
                 for r in reqs:
                     self.cached_prompt_tokens += r.cached
                     self._register(r, r.prompt_len)
-                return reqs, logits.float()
-            return reqs, self._prefill(reqs).float()
-        reqs = sorted(self._running, key=lambda r: r.sampling)
+                return reqs, logits
+            return reqs, self._prefill(reqs)
+        reqs = sorted(self._running, key=self._order)
         self._running = []
         if not reqs:
             return [], None
-        if self.cuda_graphs and len(reqs) <= self._graph_sizes[-1]:
-            return reqs, self._graph_decode(reqs).float()
-        width = max(len(r.pages) for r in reqs)
-        table = [p for r in reqs for p in r.pages + [0] * (width - len(r.pages))]
-        pos = [len(r.tokens) - 1 for r in reqs]
-        ids, positions, table = self._upload([[r.tokens[-1] for r in reqs], pos, table])
-        logits = self.model._paged_logits(ids, positions, self.k_pools, self.v_pools, table=table.view(len(reqs), width),
+        owners = [r for r in reqs for _ in r.rows()]
+        rows = [b for r in reqs for b in r.rows()]
+        if self.cuda_graphs and len(rows) <= self._graph_sizes[-1]:
+            return owners, self._graph_decode(rows)
+        width = max(len(b.pages) for b in rows)
+        table = [p for b in rows for p in b.pages + [0] * (width - len(b.pages))]
+        pos = [len(b.tokens) - 1 for b in rows]
+        ids, positions, table = self._upload([[b.tokens[-1] for b in rows], pos, table])
+        logits = self.model._paged_logits(ids, positions, self.k_pools, self.v_pools, table=table.view(len(rows), width),
                                           max_pos=max(pos), k_scales=self.k_scales, v_scales=self.v_scales)
-        return reqs, logits.float()
+        return owners, logits
 
     def _prefill(self, reqs: List[_Request]) -> torch.Tensor:
         """Whole prompts packed into one row through the document-masked flash kernel."""
@@ -491,9 +595,11 @@ class ContinuousBatcher:
         return chunks
 
     def _mixed(self) -> Tuple[List[_Request], torch.Tensor]:
-        """Chunked prefill: one decode token of every running request, then the step's prompt chunks, through one
-        forward.  Requests whose prompt completes choose their first token in this step; the others stay admitted."""
-        dec = self._running
+        """Chunked prefill: one decode token of every running request's rows (its beams, for beam search), then the
+        step's prompt chunks, through one forward.  Requests whose prompt completes choose their first token (make
+        their first beam step) from their last prompt row in this step; the others stay admitted."""
+        owners = [r for r in self._running for _ in r.rows()]
+        dec = [b for r in self._running for b in r.rows()]
         self._running = []
         chunks = self._chunks()
         width = max(len(r.pages) for r in dec + [c[0] for c in chunks])
@@ -516,8 +622,8 @@ class ContinuousBatcher:
             if self.prefix_caching:
                 self.cached_prompt_tokens += r.cached
                 self._register(r, r.prompt_len)
-        reqs = dec + done
-        order = sorted(range(len(reqs)), key=lambda i: reqs[i].sampling)      # stable: groups of equal sampling
+        reqs = owners + done
+        order = sorted(range(len(reqs)), key=lambda i: self._order(reqs[i]))  # stable: groups, each beam's rows, adjacent
         last = [rows[i] for i in order]
         n, plan = self._staging([r.pages for r, _, _ in chunks], start, [e for _, _, e in chunks])
         up = self._upload([ids, positions, table, slot, cu, start, last] + plan)
@@ -528,7 +634,7 @@ class ContinuousBatcher:
                                           cu_seqlens=cu, start=start, max_len=max(e - s for _, s, e in chunks),
                                           k_scales=self.k_scales, v_scales=self.v_scales, stage=stage,
                                           n_dec=len(dec))
-        return [reqs[i] for i in order], logits.float()
+        return [reqs[i] for i in order], logits
 
     # ------------------------------------------------------------------ CUDA graphs
     def _init_graphs(self) -> None:
@@ -595,8 +701,9 @@ class ContinuousBatcher:
         self._graphs[n] = (graph, logits, _decode_ticket(0, self.device))
         return self._graphs[n]
 
-    def _graph_decode(self, reqs: List[_Request]) -> torch.Tensor:
-        """The plain decode step by graph replay: logits ``[len(reqs), V]``, the first rows of the bucket's."""
+    def _graph_decode(self, reqs: list) -> torch.Tensor:
+        """The plain decode step by graph replay: logits ``[len(reqs), V]``, the first rows of the bucket's, for decode
+        rows ``reqs`` (requests or beams: ``tokens`` and ``pages``)."""
         n = next(s for s in self._graph_sizes if s >= len(reqs))
         graph, logits, _ = self._graph(n)
         self._graph_inputs(n, [r.tokens[-1] for r in reqs], [len(r.tokens) - 1 for r in reqs], [r.pages for r in reqs])
@@ -613,6 +720,111 @@ class ContinuousBatcher:
             picks.append(self.model._select_token(logits[i:i + n], do_sample, temperature, top_k, top_p, self.generator))
             i += n
         return torch.cat(picks).tolist()
+
+    # ------------------------------------------------------------------ beam search
+    def _beam_step(self, reqs: List[_Request], logits: torch.Tensor) -> List[Tuple[int, List[int]]]:
+        """One beam step of every beam-search request in ``reqs`` from its rows of ``logits`` (model dtype, each
+        request's rows adjacent, in ``reqs`` order), as 🤗's ``_beam_search`` makes it: the 2W best candidates
+        (``beam_topk``), finished hypotheses, the next W beams and the stopping test.  Running requests fork their
+        beams (``_fork``); one ``paged_kv_copy`` serves every copy of the step.  Returns ``(rid, prompt + best
+        hypothesis)`` of the requests that finished, whose pages are released."""
+        from pipegoose_b200.ops.attention import paged_kv_copy
+        from pipegoose_b200.ops.kernels import beam_topk, beam_topk_reference
+
+        for r in reqs:
+            if not r.beam.beams:                     # first step: the prompt's row, score 0
+                prompt = -(-r.prompt_len // PAGE_SIZE)
+                r.beam.beams = [_Beam(list(r.tokens), 0.0, r.pages[:prompt])]
+                r.beam.refs = dict.fromkeys(r.pages[:prompt], 1)
+                r.beam.spare = list(r.pages[prompt:])
+        cu, scores = [0], []
+        for r in reqs:
+            cu.append(cu[-1] + len(r.beam.beams))
+            scores += [b.score for b in r.beam.beams]
+        k = 2 * max(r.beam.width for r in reqs)
+        topk = beam_topk if self._native else beam_topk_reference
+        sc, tok, row, _ = topk(logits, torch.tensor(scores, dtype=torch.float32), cu, k)
+        host = torch.cat([sc.view(torch.int32), tok.int(), row.int()]).cpu()        # one device-to-host transfer
+        sc, tok, row = host[:len(reqs)].view(torch.float32).tolist(), host[len(reqs):2 * len(reqs)].tolist(), \
+            host[2 * len(reqs):].tolist()
+        done, copies = [], []
+        for i, r in enumerate(reqs):
+            b = r.beam
+            W = b.width
+            cands = [(sc[i][j], tok[i][j], row[i][j] - cu[i]) for j in range(2 * W)]
+            gen = len(b.beams[0].tokens) - r.prompt_len                  # tokens generated before this step
+            hit = [t == r.eos_token_id or gen + 1 >= r.max_new_tokens for _, t, _ in cands]
+            # finished hypotheses: candidates among the top W that end here, length-penalised (🤗's fp32 arithmetic)
+            if b.improvable and not (len(b.finished) == W and b.early_stopping is True):
+                div = np.float32((gen + 1) ** b.length_penalty)
+                new = [(float(np.float32(s) / div), b.beams[p].tokens[r.prompt_len:] + [t])
+                       for (s, t, p), h in zip(cands[:W], hit[:W]) if h]
+                b.finished = sorted(b.finished + new, key=lambda f: -f[0])[:W]        # stable
+            running = [c for c, h in zip(cands, hit) if not h][:W]
+            if b.improvable and len(b.finished) == W and running:
+                length = r.max_new_tokens if b.early_stopping == "never" and b.length_penalty > 0 else gen + 1
+                best = np.float32(running[0][0]) / np.float32(length ** b.length_penalty)
+                b.improvable = bool(best > np.float32(b.finished[-1][0]))
+            if all(hit) or not b.improvable or (len(b.finished) == W and b.early_stopping is True):
+                r.tokens = r.tokens[:r.prompt_len] + b.finished[0][1]
+                self.hypotheses[r.rid] = [(r.tokens[:r.prompt_len] + g, s) for s, g in
+                                          b.finished[:b.num_return_sequences]]
+                if self.prefix_caching:
+                    self._release(r)
+                else:
+                    self._free.extend(r.pages)
+                r.pages, r.beam.beams = [], []
+                done.append((r.rid, r.tokens))
+                continue
+            copies += self._fork(r, running)
+            self._running.append(r)
+        if copies:
+            paged_kv_copy(copies, self.k_pools, self.v_pools, self.k_scales, self.v_scales)
+            self.beam_page_copies += len(copies)
+        return done
+
+    def _fork(self, r: _Request, running: List[Tuple[float, int, int]]) -> List[Tuple[int, int, int]]:
+        """The request's next beams ``running`` (score, token, parent index), in 🤗's order, each taking its parent's
+        page list; returns the ``(src, dst, count)`` copies this makes.  Pages are reference-counted within the
+        request: the new beams' references are taken before the old beams' are dropped, and a page no beam holds
+        returns to the request's spare pages.  Copy-on-write: the page holding a beam's next write position
+        ``len(tokens) - 1`` must be that beam's alone.  The first of its holders in 🤗's order keeps it; every other gets
+        a spare page with the leading ``pos % 64`` slots copied.  At ``pos % 64 == 0`` the write starts a fresh page."""
+        b = r.beam
+        beams = [_Beam(b.beams[p].tokens + [t], s, list(b.beams[p].pages)) for s, t, p in running]
+        for x in beams:
+            for p in x.pages:
+                b.refs[p] += 1
+        for x in b.beams:
+            for p in x.pages:
+                b.refs[p] -= 1
+                if b.refs[p] == 0:
+                    del b.refs[p]
+                    b.spare.append(p)
+        copies, kept = [], set()
+        for x in beams:
+            k, off = divmod(len(x.tokens) - 1, PAGE_SIZE)
+            if off == 0:
+                x.pages.append(self._spare_page(r))
+                continue
+            page = x.pages[k]
+            if page not in kept:
+                kept.add(page)
+                continue
+            fresh = self._spare_page(r)
+            b.refs[page] -= 1
+            x.pages[k] = fresh
+            copies.append((page, fresh, off))
+        b.beams = beams
+        return copies
+
+    def _spare_page(self, r: _Request) -> int:
+        """One of the request's spare pages, referenced once by the beam that takes it."""
+        if not r.beam.spare:
+            raise RuntimeError(f"beam-search request {r.rid} needs more than the {len(r.pages)} pages it reserved")
+        p = r.beam.spare.pop()
+        r.beam.refs[p] = 1
+        return p
 
     # ------------------------------------------------------------------ speculative decoding
     def _draft(self, r: _Request) -> List[int]:
