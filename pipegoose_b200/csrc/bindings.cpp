@@ -737,39 +737,101 @@ void paged_kv_dequantize(const torch::Tensor& k_pool, const torch::Tensor& v_poo
                                      (int)k_pool.size(3), cur_stream()) == 0, "paged_kv_dequantize failed");
 }
 
+// KV pools as paged_kv_copy and paged_kv_swap take them: contiguous [n_layer, pages, H, 64, D] bf16, or FP8 codes with
+// fp32 scales [n_layer, pages, H, 64], on one device and 16-byte aligned.  Returns whether they are FP8 and sets the
+// bytes of one pool row.
+static bool check_kv_pools(const char* op, const torch::Tensor& k_pools, const torch::Tensor& v_pools,
+                           const c10::optional<torch::Tensor>& k_scales, const c10::optional<torch::Tensor>& v_scales,
+                           int64_t* row_bytes) {
+  PG_CUDA(k_pools); PG_CUDA(v_pools);
+  TORCH_CHECK(k_pools.dim() == 5 && v_pools.sizes() == k_pools.sizes() && k_pools.size(3) == 64 &&
+              k_pools.scalar_type() == v_pools.scalar_type() && k_pools.is_contiguous() && v_pools.is_contiguous(),
+              op, ": k_pools / v_pools must be contiguous [n_layer, pages, H, 64, D] of one dtype");
+  const bool fp8 = k_pools.scalar_type() == torch::kFloat8_e4m3fn;
+  TORCH_CHECK(fp8 || k_pools.scalar_type() == torch::kBFloat16, op, ": pools must be bf16 or float8_e4m3fn");
+  TORCH_CHECK(fp8 == k_scales.has_value() && fp8 == v_scales.has_value(),
+              op, ": float8_e4m3fn pools need k_scales and v_scales, and bf16 pools take none");
+  if (fp8) {
+    for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&*k_scales, &*v_scales}) {
+      PG_CUDA((*t)); PG_F32((*t));
+      TORCH_CHECK(t->sizes() == k_pools.sizes().slice(0, 4) && t->is_contiguous() && t->device() == k_pools.device(),
+                  op, ": scales must be contiguous fp32 [n_layer, pages, H, 64] like the pools");
+      TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, op, ": scales must be 16B aligned");
+    }
+  }
+  *row_bytes = k_pools.size(4) * k_pools.element_size();
+  TORCH_CHECK(*row_bytes % 16 == 0, op, ": a pool row of ", *row_bytes, " bytes is not a whole number of 16-byte words");
+  TORCH_CHECK(v_pools.device() == k_pools.device(), op, ": tensors on different devices");
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&k_pools, &v_pools})
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, op, ": pools must be 16B aligned");
+  return fp8;
+}
+
 // Beam-search forks: slots 0 .. count - 1 of page src into page dst, for every pair (int32 [n, 3]: src, dst, count)
 // and every layer of the pools [n_layer, pages, H, 64, D] (bf16, or FP8 codes with fp32 scales [n_layer, pages, H,
 // 64]).  The caller guarantees that every id is a page of the pools and that no dst is also a src.
 void paged_kv_copy(const torch::Tensor& pairs, torch::Tensor k_pools, torch::Tensor v_pools,
                    const c10::optional<torch::Tensor>& k_scales, const c10::optional<torch::Tensor>& v_scales) {
-  PG_CUDA(pairs); PG_CUDA(k_pools); PG_CUDA(v_pools);
+  PG_CUDA(pairs);
   TORCH_CHECK(pairs.scalar_type() == torch::kInt32 && pairs.dim() == 2 && pairs.size(1) == 3 && pairs.is_contiguous(),
               "paged_kv_copy: pairs must be contiguous int32 [n, 3] (src, dst, count)");
-  TORCH_CHECK(k_pools.dim() == 5 && v_pools.sizes() == k_pools.sizes() && k_pools.size(3) == 64 &&
-              k_pools.scalar_type() == v_pools.scalar_type() && k_pools.is_contiguous() && v_pools.is_contiguous(),
-              "paged_kv_copy: k_pools / v_pools must be contiguous [n_layer, pages, H, 64, D] of one dtype");
-  const bool fp8 = k_pools.scalar_type() == torch::kFloat8_e4m3fn;
-  TORCH_CHECK(fp8 || k_pools.scalar_type() == torch::kBFloat16, "paged_kv_copy: pools must be bf16 or float8_e4m3fn");
-  TORCH_CHECK(fp8 == k_scales.has_value() && fp8 == v_scales.has_value(),
-              "paged_kv_copy: float8_e4m3fn pools need k_scales and v_scales, and bf16 pools take none");
-  if (fp8) {
-    for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&*k_scales, &*v_scales}) {
-      PG_CUDA((*t)); PG_F32((*t));
-      TORCH_CHECK(t->sizes() == k_pools.sizes().slice(0, 4) && t->is_contiguous() && t->device() == k_pools.device(),
-                  "paged_kv_copy: scales must be contiguous fp32 [n_layer, pages, H, 64] like the pools");
-    }
-  }
-  const int64_t row_bytes = k_pools.size(4) * k_pools.element_size();
-  TORCH_CHECK(row_bytes % 16 == 0, "paged_kv_copy: a pool row of ", row_bytes, " bytes is not a whole number of 16-byte words");
-  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&pairs, &v_pools})
-    TORCH_CHECK(t->device() == k_pools.device(), "paged_kv_copy: tensors on different devices");
-  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&k_pools, &v_pools})
-    TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, "paged_kv_copy: pools must be 16B aligned");
+  int64_t row_bytes;
+  const bool fp8 = check_kv_pools("paged_kv_copy", k_pools, v_pools, k_scales, v_scales, &row_bytes);
+  TORCH_CHECK(pairs.device() == k_pools.device(), "paged_kv_copy: tensors on different devices");
   c10::cuda::CUDAGuard guard(k_pools.device());
   TORCH_CHECK(pg_paged_kv_copy(pairs.data_ptr<int>(), k_pools.data_ptr(), v_pools.data_ptr(),
                                fp8 ? k_scales->data_ptr<float>() : nullptr, fp8 ? v_scales->data_ptr<float>() : nullptr,
                                (int)pairs.size(0), (int)k_pools.size(0), (int)k_pools.size(1), (int)k_pools.size(2),
                                (int)row_bytes, cur_stream()) == 0, "paged_kv_copy failed");
+}
+
+// The device pointer of a pinned host tensor (refused if it is not pinned host memory).
+static void* pinned_device_ptr(const torch::Tensor& t, const char* what) {
+  cudaPointerAttributes attr;
+  const cudaError_t e = cudaPointerGetAttributes(&attr, t.data_ptr());
+  if (e != cudaSuccess) (void)cudaGetLastError();
+  TORCH_CHECK(e == cudaSuccess && attr.type == cudaMemoryTypeHost,
+              "paged_kv_swap: ", what, " must be in pinned host memory (Tensor.pin_memory())");
+  void* dev = nullptr;
+  const cudaError_t g = cudaHostGetDevicePointer(&dev, t.data_ptr(), 0);
+  if (g != cudaSuccess) (void)cudaGetLastError();
+  TORCH_CHECK(g == cudaSuccess && dev != nullptr, "paged_kv_swap: ", what, " has no device mapping: ",
+              cudaGetErrorString(g));
+  return dev;
+}
+
+// Preemption: K and V (and their scales over FP8 pools) of pool page `page` of every layer to or from host slot `slot`,
+// for every pair (int32 [n, 2]: page, slot).  host_kv is pinned [slots, n_layer, 2, H, 64, D] in the pools' dtype,
+// host_scales pinned fp32 [slots, n_layer, 2, H, 64] (FP8 pools only).  The caller guarantees that every id is in range.
+void paged_kv_swap(const torch::Tensor& pairs, torch::Tensor k_pools, torch::Tensor v_pools,
+                   const c10::optional<torch::Tensor>& k_scales, const c10::optional<torch::Tensor>& v_scales,
+                   torch::Tensor host_kv, const c10::optional<torch::Tensor>& host_scales, bool to_host) {
+  PG_CUDA(pairs);
+  TORCH_CHECK(pairs.scalar_type() == torch::kInt32 && pairs.dim() == 2 && pairs.size(1) == 2 && pairs.is_contiguous(),
+              "paged_kv_swap: pairs must be contiguous int32 [n, 2] (page, slot)");
+  int64_t row_bytes;
+  const bool fp8 = check_kv_pools("paged_kv_swap", k_pools, v_pools, k_scales, v_scales, &row_bytes);
+  TORCH_CHECK(pairs.device() == k_pools.device(), "paged_kv_swap: tensors on different devices");
+  const auto L = k_pools.size(0), H = k_pools.size(2), D = k_pools.size(4);
+  TORCH_CHECK(!host_kv.is_cuda() && host_kv.is_contiguous() && host_kv.scalar_type() == k_pools.scalar_type() &&
+              host_kv.dim() == 6 && host_kv.size(1) == L && host_kv.size(2) == 2 && host_kv.size(3) == H &&
+              host_kv.size(4) == 64 && host_kv.size(5) == D,
+              "paged_kv_swap: host_kv must be a contiguous host tensor [slots, n_layer, 2, H, 64, D] of the pools' dtype");
+  TORCH_CHECK(fp8 == host_scales.has_value(),
+              "paged_kv_swap: float8_e4m3fn pools need host_scales, and bf16 pools take none");
+  if (fp8)
+    TORCH_CHECK(!host_scales->is_cuda() && host_scales->is_contiguous() &&
+                host_scales->scalar_type() == torch::kFloat32 && host_scales->sizes() == host_kv.sizes().slice(0, 5),
+                "paged_kv_swap: host_scales must be a contiguous fp32 host tensor [slots, n_layer, 2, H, 64]");
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&host_kv, fp8 ? &*host_scales : &host_kv})
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, "paged_kv_swap: host tensors must be 16B aligned");
+  void* host = pinned_device_ptr(host_kv, "host_kv");
+  float* scales = fp8 ? static_cast<float*>(pinned_device_ptr(*host_scales, "host_scales")) : nullptr;
+  c10::cuda::CUDAGuard guard(k_pools.device());
+  TORCH_CHECK(pg_paged_kv_swap(pairs.data_ptr<int>(), k_pools.data_ptr(), v_pools.data_ptr(),
+                               fp8 ? k_scales->data_ptr<float>() : nullptr, fp8 ? v_scales->data_ptr<float>() : nullptr,
+                               host, scales, (int)pairs.size(0), (int)L, (int)k_pools.size(1), (int)H, (int)row_bytes,
+                               to_host ? 1 : 0, cur_stream()) == 0, "paged_kv_swap failed");
 }
 
 // Beam search's candidate choice (csrc/beam_sm90.cu): per request r (rows cu[r] .. cu[r+1] - 1 of logits [N, V], bf16
@@ -1014,6 +1076,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("v_scales"), py::arg("src"), py::arg("dst"), py::arg("k_out"), py::arg("v_out"));
   m.def("paged_kv_copy", &paged_kv_copy, py::arg("pairs"), py::arg("k_pools"), py::arg("v_pools"),
         py::arg("k_scales") = py::none(), py::arg("v_scales") = py::none());
+  m.def("paged_kv_swap", &paged_kv_swap, py::arg("pairs"), py::arg("k_pools"), py::arg("v_pools"), py::arg("k_scales"),
+        py::arg("v_scales"), py::arg("host_kv"), py::arg("host_scales"), py::arg("to_host"));
   m.def("beam_topk", &beam_topk, py::arg("logits"), py::arg("scores"), py::arg("cu"), py::arg("k"), py::arg("max_rows"),
         py::arg("out_score"), py::arg("out_token"), py::arg("out_row"), py::arg("lse"), py::arg("ticket"));
   m.def("moe_route", &moe_route);

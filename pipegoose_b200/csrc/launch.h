@@ -151,6 +151,16 @@ int pg_paged_kv_dequantize(const void* k_pool, const void* v_pool, const float* 
 int pg_paged_kv_copy(const int* pairs, void* k_pools, void* v_pools, float* k_scales, float* v_scales, int n,
                      int layers, int pages, int H, int row_bytes, cudaStream_t s);
 
+// ---- kv_swap_sm90.cu
+// Preemption: for every pair i of pairs (int32 [n, 2]: pool page, host slot), every layer, K and V of page `page` of the
+// pools [layers, pages, H, 64, D] (row_bytes = D * element size) move to or from slot `slot` of host_kv [slots, layers,
+// 2, H, 64, D] (to_host != 0: pool -> host), with the fp32 scales [layers, pages, H, 64] <-> host_scales [slots,
+// layers, 2, H, 64] when given (FP8 pools; all three or none).  host_kv / host_scales are device pointers of pinned
+// host memory (cudaHostGetDevicePointer).  The caller guarantees that every id is in range.
+int pg_paged_kv_swap(const int* pairs, void* k_pools, void* v_pools, float* k_scales, float* v_scales, void* host_kv,
+                     float* host_scales, int n, int layers, int pages, int H, int row_bytes, int to_host,
+                     cudaStream_t s);
+
 // ---- beam_sm90.cu
 // Beam search's candidate choice: for every request r (rows cu[r] .. cu[r+1] - 1 of logits [N, V], bf16 or, with
 // fp32 != 0, fp32, row stride ld) the k (1 .. 16) best (score, token, row) by score = scores[row] + (logit - lse[row]),

@@ -458,6 +458,50 @@ def paged_kv_copy(pairs, k_pools: torch.Tensor, v_pools: torch.Tensor, k_scales=
     native().paged_kv_copy(pairs, k_pools, v_pools, k_scales, v_scales)
 
 
+def _swap_pairs(pairs, pages: int, slots: int) -> torch.Tensor:
+    """``pairs`` as int32 ``[n, 2]``; a host list or CPU tensor is checked against the pool and host-pool sizes (a CUDA
+    tensor is the caller's to get right: checking it would synchronise)."""
+    pairs = (pairs if torch.is_tensor(pairs) else torch.tensor(pairs, dtype=torch.int32)).to(torch.int32).view(-1, 2)
+    if not pairs.is_cuda and pairs.numel() and not (0 <= int(pairs[:, 0].min()) and int(pairs[:, 0].max()) < pages and
+                                                    0 <= int(pairs[:, 1].min()) and int(pairs[:, 1].max()) < slots):
+        raise ValueError(f"paged_kv_swap: pairs {pairs.tolist()} outside the pool's {pages} pages or the host pool's "
+                         f"{slots} slots")
+    return pairs
+
+
+def paged_kv_swap_reference(pairs, k_pools: torch.Tensor, v_pools: torch.Tensor, k_scales, v_scales,
+                            host_kv: torch.Tensor, host_scales, to_host: bool) -> None:
+    """PyTorch form of :func:`paged_kv_swap` (bytes copied as they are, so FP8 codes move bit for bit)."""
+    fp8 = _fp8_pools(k_pools, k_scales, v_scales)
+    if fp8 != (host_scales is not None):
+        raise ValueError("float8_e4m3fn pools need host_scales, and other pools take none")
+    pools = [(k_pools, host_kv[:, :, 0]), (v_pools, host_kv[:, :, 1])]
+    if fp8:
+        pools += [(k_scales, host_scales[:, :, 0]), (v_scales, host_scales[:, :, 1])]
+    for page, slot in _swap_pairs(pairs, k_pools.shape[1], host_kv.shape[0]).tolist():
+        for pool, host in pools:
+            if to_host:
+                host[slot].copy_(pool[:, page])
+            else:
+                pool[:, page].copy_(host[slot])
+
+
+def paged_kv_swap(pairs, k_pools: torch.Tensor, v_pools: torch.Tensor, k_scales, v_scales, host_kv: torch.Tensor,
+                  host_scales, to_host: bool) -> None:
+    """Preemption: for every ``(pool page, host slot)`` of ``pairs`` (int32 ``[n, 2]`` or a host list of pairs), every
+    layer's K and V of page ``page`` of the pools ``[n_layer, pages, n_head, PAGE_SIZE, D]`` to (``to_host``) or from
+    slot ``slot`` of ``host_kv [slots, n_layer, 2, n_head, PAGE_SIZE, D]``, and over FP8 pools the scales ``[n_layer,
+    pages, n_head, PAGE_SIZE]`` to or from ``host_scales [slots, n_layer, 2, n_head, PAGE_SIZE]`` (fp32; ``None`` for
+    other pools); nothing else changes.  No page or slot may appear twice.  CUDA bf16 and FP8 pools run
+    ``paged_kv_swap_kernel``, one launch for all pairs and layers, which reads and writes the host pool (pinned: refused
+    otherwise) through its device pointer, in stream order; the host must not touch the host pool meanwhile."""
+    fp8 = _fp8_pools(k_pools, k_scales, v_scales)
+    if not (k_pools.is_cuda and (fp8 or k_pools.dtype == torch.bfloat16)):
+        return paged_kv_swap_reference(pairs, k_pools, v_pools, k_scales, v_scales, host_kv, host_scales, to_host)
+    pairs = _swap_pairs(pairs, k_pools.shape[1], host_kv.shape[0]).to(k_pools.device, non_blocking=True).contiguous()
+    native().paged_kv_swap(pairs, k_pools, v_pools, k_scales, v_scales, host_kv, host_scales, bool(to_host))
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # Prefill against paged pools (prefix caching, ``pipegoose_b200.serving``).
 #

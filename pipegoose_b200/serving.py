@@ -8,7 +8,8 @@
 The engine owns the keys and values of every layer in two pools of 64-position pages, ``[n_layer, num_pages, n_head,
 64, D]``, shared block tables for all layers and a free list.  A request is admitted first come, first served (no
 request overtakes an earlier one) as soon as ``ceil((prompt + max_new_tokens) / 64)`` pages are free; they are reserved
-until it finishes, so nothing is ever preempted, and return to the free list in the step it finishes.
+until it finishes, so nothing is ever preempted (unless ``preemption=True``: below), and return to the free list in the
+step it finishes.
 
 A step is either one prefill of newly admitted prompts, packed into one row of at most ``max_prefill_tokens`` tokens
 (a longer prompt runs alone) through the document-masked flash kernel, or one decode of every running sequence
@@ -114,6 +115,32 @@ bucket or cuBLAS's choice for another M brings, as above).  Refused: ``num_beams
 with ``num_beams > 1`` (beam sampling), ``num_return_sequences`` outside 1 .. ``num_beams``, ``2 * num_beams`` above the
 vocabulary, and beam requests on an engine with speculative decoding.
 
+Preemption (``preemption=True``, off by default; ``swap_space_tokens`` sizes a pinned host pool of whole pages and
+needs it): plain requests take pages as they grow instead of reserving their whole length.  A request is admitted with
+the pages of its tokens so far (minus prefix hits); before every decode, mixed or verify step each running plain
+request whose next write starts a page takes one off the free list.  So a request that stops at ``eos_token_id`` early
+never held the pages it did not write, and the pool holds more running requests.  When the free list cannot cover a
+step's growth, running plain requests are preempted, latest submitted first, until it can (a request may preempt
+itself; ``submit`` still refuses a request longer than the pool, so the oldest can always finish).  A victim whose pages
+fit in the free host slots is swapped out: one ``paged_kv_swap`` per step copies every such victim's pages, every layer,
+K and V (codes and scales over FP8 pools), to the host pool, and its pages are freed.  Otherwise it is recomputed: its
+pages are freed (with prefix caching ``_release`` indexes its full pages first, so its readmission mostly takes hits).
+Preempted requests wait in one queue and resume oldest first, before any waiting request is admitted: a swapped-out one
+when fresh pages for its slots are free (one ``paged_kv_swap`` per step brings back all that resume), straight into the
+running set; a recomputed one is admitted like a waiting one and prefilled over all its tokens so far, and the logits
+of its last position choose the token the skipped step would have chosen.  Admission and resumption keep enough free
+pages for the next step's growth (the next two with chunked prefill, whose steps decode too), so a request is never
+prefilled only to be thrown away in the step after.  Beam-search requests keep the whole reservation and are never
+victims; neither are admitted prompts, part-way through chunked prefill or not (they hold their prompt's pages and need
+none).  Speculative drafts never preempt: they are cut to the pages the request holds plus those the free list can
+give.  Every swap runs on the engine's stream and the host never touches the host pool, so stream order is the only
+ordering: a swap-out precedes any later write to the pages it frees, and a swap-in the forward that reads its pages.
+Works with prefix caching, FP8 pools, speculative decoding, chunked prefill, ``cuda_graphs`` and beam requests.
+``preemptions`` counts the preemptions, ``swapped_out_pages`` / ``swapped_in_pages`` the pages swapped, and
+``recomputed_tokens`` the positions prefilled again (net of prefix hits; ``cached_prompt_tokens`` counts first
+admissions only).  Swap versus recompute is chosen by host room alone, not by cost: see ``docs/KERNELS.md`` for the
+measured rates.
+
 Limits: sampled tokens depend on which requests share a step (the random stream is consumed per group; in a verify
 step a group takes one uniform number per token row, then one draw per row without the draft, then one per row);
 an ``ExpertLayer`` capacity limit counts the tokens of one step, as in ``generate()`` (with prefix caching, cached keys
@@ -122,6 +149,7 @@ rounding).  Tensor-parallel, pipelined and fused NVLink MoE models are refused.
 """
 from __future__ import annotations
 
+import bisect
 import collections
 import itertools
 from dataclasses import dataclass, field
@@ -204,6 +232,7 @@ class _Request:
     filled: int = 0            # chunked prefill: prompt positions in the cache so far (at least ``cached``)
     ngrams: Optional[_NgramIndex] = None      # speculative decoding only
     beam: Optional[_BeamSearch] = None        # beam search only
+    slots: List[int] = field(default_factory=list)   # preemption: host slots holding its pages while swapped out
 
     @property
     def pages_needed(self) -> int:
@@ -238,6 +267,10 @@ class ContinuousBatcher:
     ``cuda_graphs``: replay plain decode steps of at most ``GRAPH_BATCH_SIZES[-1]`` requests from CUDA graphs, one per
     batch bucket, captured on first use (module docstring); costs the graphs' memory pool and one capture pause per
     bucket.  Needs a model on the native decode path with ``BloomMLP`` MLPs.
+    ``preemption``: give plain requests pages as they grow instead of reserving their whole length at admission, and
+    preempt the latest submitted ones when the pool runs out (module docstring).
+    ``swap_space_tokens``: positions of the pinned host pool preempted requests are swapped into (rounded down to whole
+    pages; 0: every preempted request is recomputed).  Needs ``preemption=True``.
 
     Beam search: ``submit(..., num_beams=W)`` (module docstring); ``hypotheses`` maps a finished beam request's id to
     its best ``(prompt + tokens, score)``, and ``beam_page_copies`` counts the partial pages its forks copied."""
@@ -245,7 +278,8 @@ class ContinuousBatcher:
     def __init__(self, model, max_cache_tokens: int, max_prefill_tokens: int = 8192,
                  generator: Optional[torch.Generator] = None, prefix_caching: bool = False,
                  kv_cache_dtype: Optional[torch.dtype] = None, num_speculative_tokens: int = 0,
-                 chunked_prefill: bool = False, cuda_graphs: bool = False):
+                 chunked_prefill: bool = False, cuda_graphs: bool = False, preemption: bool = False,
+                 swap_space_tokens: int = 0):
         from pipegoose_b200.models.bloom import BloomMLP, _decodes_incrementally, _native_decode
 
         if getattr(model, "tp", None) is not None:
@@ -271,6 +305,10 @@ class ContinuousBatcher:
                              f"{PAGE_SIZE}, got {max_prefill_tokens}")
         if chunked_prefill and num_speculative_tokens:
             raise ValueError("chunked prefill does not support speculative decoding")
+        if swap_space_tokens < 0:
+            raise ValueError(f"swap_space_tokens must be at least 0, got {swap_space_tokens}")
+        if swap_space_tokens and not preemption:
+            raise ValueError("swap_space_tokens needs preemption=True: only preempted requests are swapped out")
         w = blocks[0].self_attention.query_key_value.weight
         D = model.config.hidden_size // model.config.n_head
         if cuda_graphs and not all(isinstance(b.mlp, BloomMLP) for b in blocks):
@@ -320,6 +358,20 @@ class ContinuousBatcher:
         self._waiting: collections.deque = collections.deque()    # submitted, no pages yet
         self._admitted: collections.deque = collections.deque()   # pages reserved, prompt not yet (wholly) run
         self._running: List[_Request] = []                        # prompt in the cache, decoding
+        self.preemption = bool(preemption)
+        self._preempted: List[_Request] = []                      # preempted, oldest first
+        self.preemptions = 0                                      # requests preempted (each time counts)
+        self.swapped_out_pages = 0
+        self.swapped_in_pages = 0
+        self.recomputed_tokens = 0                                # positions prefilled again, net of prefix hits
+        slots = int(swap_space_tokens) // PAGE_SIZE
+        self._host_free = collections.deque(range(slots))
+        self.host_kv = self.host_scales = None
+        if slots:
+            pin = self.device.type == "cuda"
+            self.host_kv = torch.empty((slots, shape[0], 2) + shape[2:], dtype=self.k_pools.dtype, pin_memory=pin)
+            if self.k_scales is not None:
+                self.host_scales = torch.empty((slots, shape[0], 2) + shape[2:-1], dtype=torch.float32, pin_memory=pin)
         if self.cuda_graphs:
             self._init_graphs()
 
@@ -367,12 +419,14 @@ class ContinuousBatcher:
         return r.rid
 
     def has_work(self) -> bool:
-        return bool(self._waiting or self._admitted or self._running)
+        return bool(self._waiting or self._admitted or self._running or self._preempted)
 
     def step(self) -> List[Tuple[int, List[int]]]:
         """One prefill, decode or (chunked prefill) mixed step; returns ``(rid, prompt + new tokens)`` of the requests
         that finished."""
         self._admit()
+        if self.preemption and (self.chunked_prefill or not self._admitted):
+            self._grow()
         spec = self._speculate() if self.num_speculative_tokens and not self._admitted else None
         done = []
         if spec is not None:
@@ -393,7 +447,7 @@ class ContinuousBatcher:
                 if self.prefix_caching:
                     self._release(r)
                 else:
-                    self._free.extend(r.pages)
+                    self._drop(r.pages)
                 r.pages = []
                 done.append((r.rid, r.tokens))
             else:
@@ -414,53 +468,141 @@ class ContinuousBatcher:
         return (r.beam is not None, r.sampling)
 
     def _admit(self) -> None:
-        if self.prefix_caching:
-            return self._admit_cached()
-        while self._waiting and self._waiting[0].pages_needed <= len(self._free):
-            r = self._waiting.popleft()
-            r.pages = [self._free.popleft() for _ in range(r.pages_needed)]
-            if not all(0 <= p < self.num_pages for p in r.pages):
-                raise RuntimeError(f"page ids {r.pages} outside the pool of {self.num_pages} pages")
-            self._admitted.append(r)
+        """First come, first served: no request overtakes an earlier one.  With preemption, preempted requests come
+        before waiting ones, oldest first; one ``paged_kv_swap`` brings back every swapped-out request that resumes."""
+        pairs = []
+        for queue in (self._preempted, self._waiting):
+            while queue and (self._swap_in(queue[0], pairs) if queue[0].slots else self._take(queue[0])):
+                del queue[0]
+            if queue:
+                break
+        if pairs:
+            self._swap(pairs, to_host=False)
+
+    def _take(self, r: _Request) -> bool:
+        """Admit ``r`` if the free list holds its pages: all it can need (``pages_needed``), or with preemption a plain
+        request's pages of ``tokens`` so far, plus ``_headroom``.  Prefix-cache hits take a reference; hit pages on the
+        free list count against the free pages they are taken from."""
+        hits = self._match(r) if self.prefix_caching else []
+        revived = sum(1 for p in hits if self._refs[p] == 0)
+        n = (-(-len(r.tokens) // PAGE_SIZE) if self.preemption and r.beam is None else r.pages_needed) - len(hits)
+        if n + revived + (self._headroom([r]) if self.preemption else 0) > len(self._free):
+            return False
+        for p in hits:
+            if self._refs[p] == 0:
+                del self._free[p]
+            self._refs[p] += 1
+        r.pages = hits + [self._take_page() for _ in range(n)]
+        r.cached, r.filled = len(hits) * PAGE_SIZE, 0
+        if not all(0 <= p < self.num_pages for p in r.pages):
+            raise RuntimeError(f"page ids {r.pages} outside the pool of {self.num_pages} pages")
+        if len(r.tokens) > r.prompt_len:                     # readmitted after a preemption: recomputed
+            self.recomputed_tokens += len(r.tokens) - r.cached
+        self._admitted.append(r)
+        return True
+
+    def _take_page(self) -> int:
+        """A page off the free list (with prefix caching the least recently freed one: it loses its index entry, whose
+        content is about to change, and takes one reference)."""
+        if not self.prefix_caching:
+            return self._free.popleft()
+        p = self._free.popitem(last=False)[0]
+        entry = self._page_key.pop(p, None)
+        if entry is not None:
+            del self._index[entry[0]]
+        self._refs[p] = 1
+        return p
+
+    def _drop(self, pages: List[int]) -> None:
+        """Return pages to the free list; with prefix caching drop one reference of each, last page first."""
+        if not self.prefix_caching:
+            self._free.extend(pages)
+            return
+        for p in reversed(pages):
+            self._refs[p] -= 1
+            if self._refs[p] == 0:
+                self._free[p] = None
+
+    # ------------------------------------------------------------------ preemption
+    def _headroom(self, new: List[_Request]) -> int:
+        """Pages the free list must keep so that admitting the prompts in ``new``, or resuming its swapped-out requests,
+        preempts nothing in the step that follows: those the next write of every running plain request starts (with
+        chunked prefill the next two writes: the admitting step decodes too), and those the first decode of every
+        admitted plain prompt starts (its pages hold ``len(tokens)`` positions)."""
+        ahead, n = int(self.chunked_prefill), 0
+        for r in self._running + [x for x in new if x.slots]:
+            if r.beam is None:
+                n += max(0, (len(r.tokens) - 1 + ahead) // PAGE_SIZE + 1 - len(r.pages or r.slots))
+        for r in list(self._admitted) + [x for x in new if not x.slots]:
+            n += r.beam is None and len(r.tokens) % PAGE_SIZE == 0
+        return n
+
+    def _grow(self) -> None:
+        """Before a decode, mixed or verify step: every running plain request whose next write starts a page takes one
+        off the free list.  While the free list cannot cover them, the latest submitted running plain request is
+        preempted (possibly one of them).  One ``paged_kv_swap``, enqueued before any write to the pages it frees,
+        serves the step's swap-outs."""
+        plain = sorted((r for r in self._running if r.beam is None), key=lambda r: r.rid)
+        short = {r.rid for r in plain if (len(r.tokens) - 1) // PAGE_SIZE >= len(r.pages)}
+        pairs = []
+        while len(short) > len(self._free):
+            r = plain.pop()
+            short.discard(r.rid)
+            self._preempt(r, pairs)
+        if pairs:
+            self._swap(pairs, to_host=True)
+        for r in plain:
+            if r.rid in short:
+                r.pages.append(self._take_page())
+
+    def _preempt(self, r: _Request, pairs: List[Tuple[int, int]]) -> None:
+        """Take a running request out: swap its pages out if they fit in the free host slots (their ``(page, slot)``
+        pairs join ``pairs``), else free them for a recompute (with prefix caching ``_release`` indexes its full pages
+        first, so its readmission mostly takes hits).  It waits in the preempted queue."""
+        self._running.remove(r)
+        self.preemptions += 1
+        if len(r.pages) <= len(self._host_free):
+            r.slots = [self._host_free.popleft() for _ in r.pages]
+            pairs += zip(r.pages, r.slots)
+            self.swapped_out_pages += len(r.pages)
+            self._drop(r.pages)
+        elif self.prefix_caching:
+            self._release(r)
+        else:
+            self._drop(r.pages)
+        r.pages = []
+        bisect.insort(self._preempted, r, key=lambda x: x.rid)
+
+    def _swap_in(self, r: _Request, pairs: List[Tuple[int, int]]) -> bool:
+        """Resume a swapped-out request if fresh pages for its slots, plus ``_headroom``, are free: its ``(page, slot)``
+        pairs join ``pairs`` and it rejoins the running set."""
+        if len(r.slots) + self._headroom([r]) > len(self._free):
+            return False
+        r.pages = [self._take_page() for _ in r.slots]
+        pairs += zip(r.pages, r.slots)
+        self._host_free.extend(r.slots)
+        self.swapped_in_pages += len(r.slots)
+        r.slots = []
+        self._running.append(r)
+        return True
+
+    def _swap(self, pairs: List[Tuple[int, int]], to_host: bool) -> None:
+        from pipegoose_b200.ops.attention import paged_kv_swap
+
+        paged_kv_swap(pairs, self.k_pools, self.v_pools, self.k_scales, self.v_scales, self.host_kv, self.host_scales,
+                      to_host)
 
     # ------------------------------------------------------------------ prefix cache
     def _match(self, r: _Request) -> List[int]:
         """Indexed pages holding the prompt's leading full pages, at most ``(prompt - 1) // 64``."""
         hits, parent = [], -1
-        for k in range((r.prompt_len - 1) // PAGE_SIZE):
+        for k in range((len(r.tokens) - 1) // PAGE_SIZE):
             page = self._index.get((parent, tuple(r.tokens[k * PAGE_SIZE:(k + 1) * PAGE_SIZE])))
             if page is None:
                 break
             hits.append(page)
             parent = self._page_key[page][1]
         return hits
-
-    def _admit_cached(self) -> None:
-        """First come, first served; hit pages on the free list count against the free pages they are taken from."""
-        while self._waiting:
-            r = self._waiting[0]
-            hits = self._match(r)
-            revived = sum(1 for p in hits if self._refs[p] == 0)
-            if r.pages_needed - len(hits) > len(self._free) - revived:
-                return
-            self._waiting.popleft()
-            for p in hits:
-                if self._refs[p] == 0:
-                    del self._free[p]
-                self._refs[p] += 1
-            fresh = []
-            for _ in range(r.pages_needed - len(hits)):
-                p = self._free.popitem(last=False)[0]                    # least recently freed
-                entry = self._page_key.pop(p, None)
-                if entry is not None:                                    # evicted: its content is about to change
-                    del self._index[entry[0]]
-                self._refs[p] = 1
-                fresh.append(p)
-            r.pages = hits + fresh
-            r.cached = len(hits) * PAGE_SIZE
-            if not all(0 <= p < self.num_pages for p in r.pages):
-                raise RuntimeError(f"page ids {r.pages} outside the pool of {self.num_pages} pages")
-            self._admitted.append(r)
 
     def _register(self, r: _Request, filled: int) -> None:
         """Index the request's full pages among positions ``0 .. filled-1`` (all written to the pools).  A key that is
@@ -484,10 +626,7 @@ class ContinuousBatcher:
         """A finished request: index the pages its generated tokens filled (positions up to ``len(tokens) - 2`` are in
         the cache; a beam-search request indexes its prompt only), then drop its references, last page first."""
         self._register(r, r.prompt_len if r.beam is not None else len(r.tokens) - 1)
-        for p in reversed(r.pages):
-            self._refs[p] -= 1
-            if self._refs[p] == 0:
-                self._free[p] = None
+        self._drop(r.pages)
 
     def _upload(self, rows: List[List[int]]) -> List[torch.Tensor]:
         """Host int lists -> int32 device tensors, in one copy."""
@@ -501,16 +640,17 @@ class ContinuousBatcher:
             return self._mixed()
         if self._admitted:                                      # prefill the oldest admitted prompts
             reqs, n = [], 0
-            while self._admitted and (not reqs or n + self._admitted[0].prompt_len - self._admitted[0].cached
+            while self._admitted and (not reqs or n + len(self._admitted[0].tokens) - self._admitted[0].cached
                                       <= self.max_prefill_tokens):
                 reqs.append(self._admitted.popleft())
-                n += reqs[-1].prompt_len - reqs[-1].cached
+                n += len(reqs[-1].tokens) - reqs[-1].cached
             reqs.sort(key=self._order)
             if self.prefix_caching:
                 logits = self._prefill_cached(reqs) if any(r.cached for r in reqs) else self._prefill(reqs)
                 for r in reqs:
-                    self.cached_prompt_tokens += r.cached
-                    self._register(r, r.prompt_len)
+                    if len(r.tokens) == r.prompt_len:            # a first admission, not a recompute
+                        self.cached_prompt_tokens += r.cached
+                    self._register(r, len(r.tokens))
                 return reqs, logits
             return reqs, self._prefill(reqs)
         reqs = sorted(self._running, key=self._order)
@@ -533,7 +673,7 @@ class ContinuousBatcher:
         """Whole prompts packed into one row through the document-masked flash kernel."""
         ids, positions, seg, slot, last, o = [], [], [], [], [], 0
         for r in reqs:
-            P = r.prompt_len
+            P = len(r.tokens)
             ids += r.tokens
             positions += range(P)
             seg += [o] * P
@@ -551,7 +691,7 @@ class ContinuousBatcher:
         width = max(len(r.pages) for r in reqs)
         table = []
         for r in reqs:
-            P, st = r.prompt_len, r.cached
+            P, st = len(r.tokens), r.cached
             ids += r.tokens[st:P]
             positions += range(st, P)
             slot += [r.pages[p // PAGE_SIZE] * PAGE_SIZE + p % PAGE_SIZE for p in range(st, P)]
@@ -560,8 +700,8 @@ class ContinuousBatcher:
             cu.append(o)
             start.append(st)
             table += r.pages + [0] * (width - len(r.pages))
-        max_len = max(r.prompt_len - r.cached for r in reqs)
-        n, plan = self._staging([r.pages for r in reqs], [r.cached for r in reqs], [r.prompt_len for r in reqs])
+        max_len = max(len(r.tokens) - r.cached for r in reqs)
+        n, plan = self._staging([r.pages for r in reqs], [r.cached for r in reqs], [len(r.tokens) for r in reqs])
         up = self._upload([ids, positions, slot, last, cu, start, table] + plan)
         ids, positions, slot, last, cu, start, table = up[:7]
         stage = (n, up[7], up[8], up[9], up[10].view(len(reqs), -1)) if plan else None
@@ -586,11 +726,12 @@ class ContinuousBatcher:
         for r in self._admitted:
             s = max(r.filled, r.cached)
             room = self.max_prefill_tokens - n
-            e = r.prompt_len if r.prompt_len - s <= room else (s + room) // PAGE_SIZE * PAGE_SIZE
+            P = len(r.tokens)
+            e = P if P - s <= room else (s + room) // PAGE_SIZE * PAGE_SIZE
             if e > s:
                 chunks.append((r, s, e))
                 n += e - s
-            if e < r.prompt_len:
+            if e < P:
                 break
         return chunks
 
@@ -614,14 +755,15 @@ class ContinuousBatcher:
             cu.append(cu[-1] + e - s)
             start.append(s)
             r.filled = e
-            if e == r.prompt_len:
+            if e == len(r.tokens):
                 done.append(r)
                 rows.append(len(dec) + cu[-1] - 1)
         for r in done:                                          # the oldest admitted requests
             self._admitted.popleft()
             if self.prefix_caching:
-                self.cached_prompt_tokens += r.cached
-                self._register(r, r.prompt_len)
+                if len(r.tokens) == r.prompt_len:                # a first admission, not a recompute
+                    self.cached_prompt_tokens += r.cached
+                self._register(r, len(r.tokens))
         reqs = owners + done
         order = sorted(range(len(reqs)), key=lambda i: self._order(reqs[i]))  # stable: groups, each beam's rows, adjacent
         last = [rows[i] for i in order]
@@ -772,7 +914,7 @@ class ContinuousBatcher:
                 if self.prefix_caching:
                     self._release(r)
                 else:
-                    self._free.extend(r.pages)
+                    self._drop(r.pages)
                 r.pages, r.beam.beams = [], []
                 done.append((r.rid, r.tokens))
                 continue
@@ -829,7 +971,8 @@ class ContinuousBatcher:
     # ------------------------------------------------------------------ speculative decoding
     def _draft(self, r: _Request) -> List[int]:
         """Prompt-lookup drafts of a running request, at most ``max_new_tokens - generated - 1`` of them so that every
-        position the step writes lies in the pages reserved at admission."""
+        position the step writes lies in the pages reserved at admission (with preemption ``_speculate`` cuts them to
+        the pages the request holds and the free list can give)."""
         if r.ngrams is None:
             r.ngrams = _NgramIndex()
         r.ngrams.update(r.tokens)
@@ -842,6 +985,11 @@ class ContinuousBatcher:
         step is then the plain decode step."""
         reqs = sorted(self._running, key=lambda r: r.sampling)
         drafts = [self._draft(r) for r in reqs]
+        if self.preemption:                          # drafts take free pages but never preempt
+            for i, r in enumerate(reqs):
+                drafts[i] = d = drafts[i][:max(0, (len(r.pages) + len(self._free)) * PAGE_SIZE - len(r.tokens))]
+                while len(r.pages) * PAGE_SIZE < len(r.tokens) + len(d):
+                    r.pages.append(self._take_page())
         if not any(drafts):
             return None
         self._running = []
